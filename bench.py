@@ -1,4 +1,4 @@
-"""bench.py -- pods scheduled/sec (and consolidation candidates/sec) of the B200 solver on BASELINE.json's configs.
+"""bench.py -- pods scheduled/sec (and consolidation candidates/sec) of the H100 solver on BASELINE.json's configs.
 
 A step == one Scheduler.Solve over the whole synthetic batch.
   N = 1  headline = configs[2] (C3), the largest single-GPU configuration: 1 000 000 pods = 1 000 apps x 1 000 replicas,
@@ -15,7 +15,9 @@ A step == one Scheduler.Solve over the whole synthetic batch.
          collective of the job -- the library's ncclAllReduce of the global topology-domain counter table -- inside
          the CUDA-event window.  Total work is fixed: "scaling": "strong".
 `--impl reference` times the CPU restatement of the reference algorithm (oracle/, kind "port": the Go reference
-cannot be built in this image) on the box's host cores, on a bounded sample of the same workload.
+is not built by this project) on the box's host cores, on a bounded sample of the same workload.
+`--dump-outputs DIR` writes the arrays the timed calls returned in their last step (headline and consolidation) as
+DIR/<section>.<key>.npy, for output-by-output comparison of two builds on the same seeded inputs.
 """
 import argparse
 import json
@@ -49,17 +51,42 @@ def algorithmic_bytes(res, n_pods, n_its, n_groups=0, domains=4):
     return n_pods * B_POD + ev * B_CLAIM + res["n_commits"] * B_CLAIM + n_its * B_IT + 2 * n_groups * domains * 4
 
 
-def ncu_traffic(key):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one solver launch on this workload, from the tracked ncu capture
-    (profiles/r2_ncu_traffic.json; a number measured under a profiler is evidence, not a bench value); None if absent."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_traffic.json"))).get(key)
-    except Exception:
-        return None
+DUMP_ARRAY_BYTES = 4 << 20  # one dumped array; larger outputs are written as a seeded sample of their rows
+DUMP_TOTAL_BYTES = 64 << 20
+DUMPED = [0]  # bytes written by dump_outputs in this run
+
+
+def _as_float(a):
+    f = a.astype(np.float32)
+    return f if np.array_equal(f.astype(a.dtype), a) else a.astype(np.float64)
+
+
+def dump_outputs(out_dir, section, arrays):
+    """Write `arrays` (name -> array or scalar) as out_dir/<section>.<name>.npy in float32 where that is exact, else float64.
+    A 64-bit integer (bit mask, quantity, range bound) becomes its two 32-bit halves on a new last axis (low, high), so
+    every value survives.  An array above DUMP_ARRAY_BYTES keeps a sample of its rows drawn with a fixed seed; the row
+    indices go to <section>.<name>.rows.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.atleast_1d(np.asarray(a))
+        if a.dtype.kind in "iu" and a.dtype.itemsize == 8:
+            a = np.ascontiguousarray(a).view(np.uint32).reshape(a.shape + (2,))
+        f = _as_float(a)
+        if f.nbytes > DUMP_ARRAY_BYTES:
+            k = max(1, DUMP_ARRAY_BYTES // (f.nbytes // len(f)) - 1)
+            rows = np.sort(np.random.default_rng(0).choice(len(f), size=k, replace=False))
+            f = f[rows]
+            rows = _as_float(rows)
+            np.save(os.path.join(out_dir, f"{section}.{name}.rows.npy"), rows)
+            DUMPED[0] += rows.nbytes
+        np.save(os.path.join(out_dir, f"{section}.{name}.npy"), f)
+        DUMPED[0] += f.nbytes
+    if DUMPED[0] > DUMP_TOTAL_BYTES:
+        raise RuntimeError(f"--dump-outputs wrote {DUMPED[0]} bytes, above {DUMP_TOTAL_BYTES}")
 
 
 class ClockSampler(threading.Thread):
-    """SM clock and throttle reasons while the timed region runs (B200_PROFILING.md).  Sampled through NVML in-process:
+    """SM clock and throttle reasons while the timed region runs.  Sampled through NVML in-process:
     spawning `nvidia-smi` five times a second stalls a one-warp kernel for hundreds of milliseconds at a time (measured:
     individual steps went from 189 ms to 0.5 - 1.4 s), an NVML query does not.  Falls back to nvidia-smi at 1 Hz."""
 
@@ -257,9 +284,9 @@ def time_encoder(n_pods_headline, e2e_ms):
 
 def peak_gbs():
     try:
-        return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", 6650.0), "measured"
+        return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", 3350.0), "measured"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 def time_provisioning(h, problem, n_pods, steps, warmup, torch, flush, barrier, sampler=None, e2e_steps=None):
@@ -297,12 +324,12 @@ def time_provisioning(h, problem, n_pods, steps, warmup, torch, flush, barrier, 
             "launches_per_step": int(launches), "e2e_ms": 1000 * float(np.mean(e2e_t)), "stats": st, "res": res}
 
 
-def roofline_block(res, n_pods, n_its, ms, key):
+def roofline_block(res, n_pods, n_its, ms):
     peak, src = peak_gbs()
     balg = algorithmic_bytes(res, n_pods, n_its, res["n_groups"])
     achieved = balg / (ms / 1000) / 1e9
     return {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": ncu_traffic(key), "kernel": "k_wsolve", "peak_source": src, "algorithmic_bytes": int(balg),
+            "kernel": "k_wsolve", "peak_source": src, "algorithmic_bytes": int(balg),
             "note": "B_alg = bytes the REFERENCE algorithm moves on this input (SURVEY 8d); k_wsolve is a latency-bound "
                     "serial first-fit chain (one warp per Scheduler) that skips provably failing candidates, so its "
                     "DRAM traffic is a few MB and the fraction measures chain speed, not bandwidth use; see DESIGN.md"}
@@ -319,14 +346,14 @@ def run_consolidation(args, h, rank, world, dist, torch):
     ci = _abi.ConsolInput(**sharding.shard_subsets(consol, rank, world))
     dev_ms, e2e_ms = [], []
     res = None
-    for i in range(1 + max(1, min(args.steps, 3))):
+    for i in range(args.warmup + args.steps):
         torch.cuda.synchronize()
         if dist is not None:
             dist.barrier()
         t0 = time.perf_counter()
         res = h.consolidate(enc.problem, ci)  # host buffers in, decisions out: upload + kernels + download
         torch.cuda.synchronize()
-        if i >= 1:
+        if i >= args.warmup:
             e2e_ms.append(1000 * (time.perf_counter() - t0))
             dev_ms.append(res["solve_ms"])
     ms, e2e = float(np.mean(dev_ms)), float(np.mean(e2e_ms))
@@ -340,20 +367,18 @@ def run_consolidation(args, h, rank, world, dist, torch):
         decisions = dt.cpu().numpy()
     if rank != 0:
         return None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, "consolidation", {k: res[k] for k in _abi.CONSOL_PARITY_KEYS})
     E = args.consol_nodes
     pods_per = (consol["node_pod_off"][1:] - consol["node_pod_off"][:-1])
     pods_sub = np.add.reduceat(pods_per[nodes], off[:-1])
     balg = int(pods_sub.sum()) * B_POD + int(((E - (off[1:] - off[:-1])) * pods_sub).sum()) * B_CLAIM  # SURVEY.md 8(d)
     peak, src = peak_gbs()
-    traffic = ncu_traffic("c4_k_consolidate")
     roof = {"bound": "hbm", "peak": peak, "unit": "GB/s", "peak_source": src, "kernel": "k_consolidate",
-            "traffic": traffic, "reference_algorithm_bytes": int(balg),
+            "reference_algorithm_bytes": int(balg),
             "note": "the reference re-reads every node row per pod per subset (reference_algorithm_bytes); "
                     "k_consolidate reads per-class candidate bitmaps and keeps per-subset state on chip, so the honest "
-                    "roofline is its own DRAM traffic (ncu dram__bytes, profiles/) over its device time"}
-    if traffic:
-        roof["achieved"] = traffic / (ms / 1000) / 1e9
-        roof["frac"] = roof["achieved"] / peak
+                    "roofline is its own DRAM traffic over its device time (not measured here)"}
     out = {"metric": "consolidation candidates/sec", "value": S / (ms / 1000), "unit": "subsets/s", "ms": ms,
            "workload": "C4: 10 000 existing KWOK nodes holding 200 000 running pods (bin-packed, 99 % of vCPU requested), "
                        "every <=3-node subset of the 100 nodes with the lowest disruption cost",
@@ -469,6 +494,7 @@ def main():
     ap.add_argument("--no-c5", action="store_true")
     ap.add_argument("--consol-nodes", type=int, default=10_000)
     ap.add_argument("--consol-pods", type=int, default=200_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's result arrays as DIR/<section>.<key>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -478,12 +504,12 @@ def main():
         return
     import torch
     import torch.distributed as dist
-    from karpenter_b200 import _native, workloads
+    from karpenter_b200 import _abi, _native, workloads
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     h = _native.Handle(local_rank)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -496,11 +522,13 @@ def main():
               " (+ counter scatter + ncclAllReduce when sharded), max over ranks")
     line = None
     if world == 1:
-        # ---------------- headline: C3 at BASELINE size on one B200
+        # ---------------- headline: C3 at BASELINE size on one H100
         enc = workloads.config_c3(n_apps=args.apps, replicas=C3_REPLICAS, n_its=C3_ITS)
         n_pods = args.apps * C3_REPLICAS
         m = time_provisioning(h, enc.problem, n_pods, args.steps, args.warmup, torch, flush, barrier, sampler)
         res, st = m["res"], m["stats"]
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, "c3", {k: res[k] for k in _abi.PARITY_KEYS})
         name = C3_NAME if args.apps == C3_APPS else C3_NAME.replace("1M pods = 1000 apps", f"{n_pods} pods = {args.apps} apps")
         line = {
             "metric": "pods scheduled/sec", "value": n_pods / (m["ms"] / 1000), "unit": "pods/s", "n_gpus": 1,
@@ -513,7 +541,7 @@ def main():
                     "host_prep_ms": st["prep_ms"], "upload_ms": st["upload_ms"], "kernels_ms": st["solve_ms"],
                     "download_ms": st["download_ms"]},
             "gpu_launches": m["launches_per_step"] * args.steps,
-            "roofline": roofline_block(res, n_pods, C3_ITS, m["ms"], "c3_k_wsolve"),
+            "roofline": roofline_block(res, n_pods, C3_ITS, m["ms"]),
             "clocks": sampler.summary(),
             "unscheduled": int((res["pod_target"] == -1).sum()), "node_claims": int(res["n_claims"]),
             "us_per_pod": 1000 * m["ms"] / n_pods, "wall_s_timed_region": m["wall"], "ms_per_step_all": m["ms_all"],
@@ -541,7 +569,7 @@ def main():
                   "us_per_pod": 1000 * m2["ms"] / C2_PODS, "ms_per_step_all": m2["ms_all"],
                   "e2e": {"value": C2_PODS / (m2["e2e_ms"] / 1000), "unit": "pods/s", "ms_per_step": m2["e2e_ms"],
                           "h2d_bytes_per_step": int(st2["bytes_h2d"]), "d2h_bytes_per_step": int(st2["bytes_d2h"])},
-                  "roofline": roofline_block(m2["res"], C2_PODS, C2_ITS, m2["ms"], "c2_k_wsolve"),
+                  "roofline": roofline_block(m2["res"], C2_PODS, C2_ITS, m2["ms"]),
                   "unscheduled": int((m2["res"]["pod_target"] == -1).sum()), "node_claims": int(m2["res"]["n_claims"])}
             if not args.no_cpu_baseline:
                 t0 = time.perf_counter()
@@ -554,7 +582,8 @@ def main():
         # ---------------- secondary: a Deployment-shaped queue (cohort commits) and the Python encoder on Pod objects
         if not args.no_deployments:
             encd = workloads.config_deployments(C3_APPS, C3_REPLICAS, n_its=C3_ITS, topology=True)
-            md = time_provisioning(h, encd.problem, n_pods_dep := C3_APPS * C3_REPLICAS, 2, 1, torch, flush, barrier, e2e_steps=1)
+            md = time_provisioning(h, encd.problem, n_pods_dep := C3_APPS * C3_REPLICAS, args.steps, args.warmup, torch, flush, barrier,
+                                   e2e_steps=1)
             line["deployments"] = {
                 "workload": "NOT a BASELINE config: 1 000 Deployments x 1 000 identical replicas with C3's constraints (zonal spread + "
                             "hostname anti-affinity), every Deployment with its own CPU request so that its pods stand together in the "
@@ -565,7 +594,7 @@ def main():
             line["encoder"] = time_encoder(n_pods, m["e2e_ms"])
         # ---------------- secondary: C5's 8 NodePool shards as one batch on this GPU
         if not args.no_c5:
-            m5 = time_c5(h, 0, 1, 1, 1, torch, None, flush, barrier)
+            m5 = time_c5(h, 0, 1, args.steps, args.warmup, torch, None, flush, barrier)
             line["c5_one_gpu"] = {
                 "workload": C5_NAME.replace("NodePool p on rank p mod N", "all 8 NodePool shards as ONE kp_solve_batch on this GPU, one CTA each"),
                 "value": m5["n_total"] / (m5["ms"] / 1000), "unit": "pods/s", "ms_per_step": m5["ms"], "n_pods": m5["n_total"],
@@ -607,6 +636,8 @@ def main():
                            device="cuda", dtype=torch.int64)
         dist.all_reduce(agg)
         claims, unsched, n_all, h2d, d2h, evs, commits, ngroups = [int(x) for x in agg.tolist()]
+        if rank == 0 and args.dump_outputs:  # NodePool 0's shard (rank 0 solves it)
+            dump_outputs(args.dump_outputs, "c5_pool0", {k: m5["outs"][0][k] for k in _abi.PARITY_KEYS})
         if rank == 0:
             assert n_all == m5["n_total"], (n_all, m5["n_total"])
             peak, src = peak_gbs()

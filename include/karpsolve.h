@@ -1,4 +1,4 @@
-/* karpsolve.h -- C ABI of libkarpsolve.so: the B200 solver behind Karpenter's
+/* karpsolve.h -- C ABI of libkarpsolve.so: the H100 solver behind Karpenter's
  * provisioning hot path.
  *
  * What this boundary replaces (all paths relative to the reference tree,

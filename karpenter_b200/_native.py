@@ -24,7 +24,7 @@ class SolverError(RuntimeError):
 
 
 def build(verbose=False):
-    """Compile every CUDA source for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile every CUDA source for sm_90a (nvcc cross-compiles without a GPU)."""
     out = subprocess.run(["make", "-C", CSRC], capture_output=True, text=True)
     if out.returncode != 0:
         raise RuntimeError("building libkarpsolve.so failed:\n" + out.stdout[-4000:] + out.stderr[-4000:])

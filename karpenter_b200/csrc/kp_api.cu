@@ -154,6 +154,7 @@ static bool nccl_load(std::string& err) {
 
 struct kp_handle {
   int device = 0;
+  int n_sm = 132;  // SMs of the device (kp_create); 132 on an H100 SXM
   cudaStream_t stream = nullptr;
   std::string err;
   Arena arena;
@@ -290,7 +291,7 @@ static void batch_clear(kp_handle* h);
 
 extern "C" {
 
-#define KP_TRUNC_BLOCKS 148  // k_truncate_claims: 4 warps per block, one claim per warp at a time
+#define KP_TRUNC_BLOCKS 132  // k_truncate_claims: one block per H100 SM, 4 warps per block, one claim per warp at a time
 int kp_version(void) { return KP_ABI_VERSION; }
 
 // sort.Slice order of a key array (host; no device needed): see kp_gosort_host.hpp
@@ -320,6 +321,7 @@ int kp_create(int device, kp_handle** out) {
   cudaEventCreate(&h->ev1);
   cudaEventCreate(&h->ev2);
   cudaEventCreate(&h->ev3);
+  cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device);
   cudaDeviceSetLimit(cudaLimitStackSize, 16384);  // pdqsort emulation recurses (log n deep)
   *out = h;
   return KP_OK;
@@ -1527,7 +1529,7 @@ int kp_feasibility(kp_handle* h, const kp_problem* p, uint64_t* out_bits, int32_
   if (d.N > 0) k_feasibility<<<(d.N * 32 + 255) / 256, 256, 0, h->stream>>>(d, nullptr, 1);
   CK(cudaEventRecord(h->ev0, h->stream));
   if (d.N > 0 && d.X > 0) {
-    int blocks = 148 * 8;
+    int blocks = h->n_sm * 8;
     k_feasibility<<<blocks, 256, 0, h->stream>>>(d, dout, 0);
   }
   CK(cudaEventRecord(h->ev1, h->stream));
@@ -1774,7 +1776,7 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
     // solved by ONE k_wsolve_batch launch (one CTA per set), then k_decide_batch applies computeConsolidation.
     double total_ms = 0;
     bool timed_out = false;
-    const int CHUNK = 296;  // two waves of 148 SMs; bounds the HBM the side-by-side tables take
+    const int CHUNK = 2 * h->n_sm;  // two waves of CTAs; bounds the HBM the side-by-side tables take
     std::vector<uint8_t> is_cand(std::max(E, 1), 0), flags(std::max(E, 1), 0);
     for (int c0 = 0; c0 < S && !timed_out; c0 += CHUNK) {
       const int c1 = std::min(S, c0 + CHUNK);
@@ -1997,14 +1999,13 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   size_t smem = fixed + tb + 64;
   const bool lean = !t.has_bounds && !t.min_values_strict && t.n_rsv == 0 && d.n_hostports == 0 && !getenv("KP_NO_LEAN");  // (G == 0 here)
   CK(cudaFuncSetAttribute(lean ? k_consolidate<true> : k_consolidate<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_sm = 1, n_sm = 148;
+  int per_sm = 1;
   if (lean)
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_consolidate<true>, CONSOL_WARPS * 32, smem);
   else
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_consolidate<false>, CONSOL_WARPS * 32, smem);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->device);
   per_sm = std::max(per_sm, 1);
-  int grid = std::min(n_sm * per_sm, std::max(1, (S + CONSOL_WARPS - 1) / CONSOL_WARPS));
+  int grid = std::min(h->n_sm * per_sm, std::max(1, (S + CONSOL_WARPS - 1) / CONSOL_WARPS));
   const size_t slots = (size_t)grid * CONSOL_WARPS, cq = (size_t)capq;
   CK(zeros(h, &q.queue, slots * (cq + 1)));
   CK(zeros(h, &q.qcls, slots * (cq + 1)));

@@ -1,4 +1,4 @@
-// kp_kernels.cuh -- device code of the solver (sm_100a).
+// kp_kernels.cuh -- device code of the solver (sm_90a).
 //
 //   k_feasibility  (K1)  class x template instance-type feasibility bitmaps: one warp per (class, template) pair,
 //                        bit-sliced mask ANDs -- filterInstanceTypesByRequirements (nodeclaim.go:412-480).

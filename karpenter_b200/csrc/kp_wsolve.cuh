@@ -1,8 +1,8 @@
 // kp_wsolve.cuh -- the Scheduler.Solve loop (scheduler.go:381-684) executed by ONE WARP per Scheduler instance.
 //
 // First-fit-decreasing with the reference's "fewest pods first" claim order is a serial chain: pod i's placement
-// decides the state pod i+1 sees.  A CTA-wide design spends its time in barriers around one working warp (ncu:
-// profiles/r1_v3_*), so the chain runs inside a single warp with no block-level synchronisation at all:
+// decides the state pod i+1 sees.  A CTA-wide design spends its time in barriers around one working warp, so the
+// chain runs inside a single warp with no block-level synchronisation at all:
 //
 //   lane k  owns label key k      (requirement slot algebra: Compatible / Add)
 //   lane r  owns resource r       (requests, Fits)

@@ -5,7 +5,7 @@
 //   scheduler.go:504 (newNodeClaims by len(Pods)), queue.go:38, cloudprovider/types.go:240 (OrderByPrice),
 //   disruption/consolidation.go:127 (sortCandidates)
 // and the permutation it leaves among EQUAL keys decides which NodeClaim a pod lands on (SURVEY.md H2).
-// The Go standard library is not part of /root/reference (third-party: Go toolchain go1.26.3 per go.mod), so this
+// The Go standard library is not part of the reference repository (third-party: Go toolchain go1.26.3 per go.mod), so this
 // follows the published algorithm; tie-order parity against a real Go run is UNPINNED (no reference test asserts it).
 #pragma once
 #include <cstdint>

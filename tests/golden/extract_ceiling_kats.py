@@ -1,15 +1,16 @@
 """Extracts the request-ceiling known-answer tests of the reference (pkg/utils/resources/suite_test.go:40-651, "Resource
 Calculations") into tests/golden/ceiling_kats.json: for every It(...) the pod (container requests / limits, init
 containers in order with their restart policy, RuntimeClass overhead, pod-level resources) and the expected
-resources.Ceiling(pod).Requests / .Limits.  Run in the build container (reads /root/reference); the JSON is committed.
+resources.Ceiling(pod).Requests / .Limits.  Run against a checkout of the reference; the JSON is committed.
 
-    python tests/golden/extract_ceiling_kats.py
+    python tests/golden/extract_ceiling_kats.py <reference checkout>
 """
 import json
 import os
 import re
+import sys
 
-SRC = "/root/reference/pkg/utils/resources/suite_test.go"
+SRC = os.path.join(sys.argv[1], "pkg/utils/resources/suite_test.go")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "ceiling_kats.json")
 
 

@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
 """Extract the reference's known-answer tables for the requirement algebra into tests/golden/requirement_kats.json.
 
-Sources (read-only, only present in the authoring container):
-  /root/reference/pkg/scheduling/requirement_test.go   Intersection tables (with / without minValues), Has, Operator, Len
-  /root/reference/pkg/scheduling/requirements_test.go  Compatible matrices (AllowUndefinedWellKnownLabels and strict)
+Sources, in a checkout of the reference given as the first argument:
+  pkg/scheduling/requirement_test.go    Intersection tables (with / without minValues), Has, Operator, Len
+  pkg/scheduling/requirements_test.go   Compatible matrices (AllowUndefinedWellKnownLabels and strict)
 
 The Go sources are parsed textually: `name := NewRequirement[WithFlexibility](key, op, [minValues,] values...)`
 definitions build a symbol table; `Entry(nil, a, b, expected)` rows and `Expect(a.Compatible(b[, opt])).To[Not](Succeed())`
@@ -13,7 +13,7 @@ import json
 import re
 import sys
 
-REF = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+REF = sys.argv[1]
 OPS = {"NodeSelectorOpIn": "In", "NodeSelectorOpNotIn": "NotIn", "NodeSelectorOpExists": "Exists",
        "NodeSelectorOpDoesNotExist": "DoesNotExist", "NodeSelectorOpGt": "Gt", "NodeSelectorOpLt": "Lt",
        "NodeSelectorOpGte": "Gte", "NodeSelectorOpLte": "Lte"}

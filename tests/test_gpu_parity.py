@@ -242,7 +242,7 @@ def test_solve_batch_matches_single_solves(handle):
 
 
 def test_solve_batch_more_instances_than_sms(handle):
-    """200 instances > 148 SMs: the launch runs in waves; results are per-instance exact."""
+    """200 instances > 132 SMs: the launch runs in waves; results are per-instance exact."""
     encs = [workloads.config_c1(n_pods=20 + 3 * i) for i in range(200)]
     outs = handle.solve_batch([e.problem for e in encs])
     for i in (0, 57, 148, 199):

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Derive karpenter_b200/data/aws_instance_types.tsv from the reference's KWOK example catalog
-(/root/reference/kwok/examples/aws_instance_types.json, 1724 entries x 8 offerings).
+(kwok/examples/aws_instance_types.json of the reference, 1724 entries x 8 offerings; its path is the first argument).
 
 The catalog is benchmark INPUT DATA (SURVEY.md section 8(d): configs C2/C3/C5 use its first 500 / 1000 entries); the
 reference tree is not present on the GPU box, so the regular structure (4 zones x {spot, on-demand}, one on-demand and
@@ -10,7 +10,7 @@ Run here (authoring container), commit the output.
 import json
 import sys
 
-SRC = sys.argv[1] if len(sys.argv) > 1 else "/root/reference/kwok/examples/aws_instance_types.json"
+SRC = sys.argv[1]
 DST = sys.argv[2] if len(sys.argv) > 2 else "karpenter_b200/data/aws_instance_types.tsv"
 ZONES = ["us-west-2a", "us-west-2b", "us-west-2c", "us-west-2d"]
 

@@ -2,7 +2,7 @@
 """Attribute the warp-stall samples of an ncu report to CUDA source lines.
 
     ncu -i prof.ncu-rep --page source --csv > prof_sass.csv
-    cuobjdump -xelf all libkarpsolve.so ; nvdisasm -g -c kp_api.sm_100a.cubin > k.sass
+    cuobjdump -xelf all libkarpsolve.so ; nvdisasm -g -c kp_api.sm_90a.cubin > k.sass
     python tools/ncu_lines.py prof_sass.csv k.sass k_solve [top]
 
 ncu's CSV source page is per SASS instruction; nvdisasm -g interleaves `//## File "...", line N` markers with the same

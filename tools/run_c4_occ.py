@@ -1,9 +1,7 @@
 """C4 consolidation with the stock library (2 CTAs / SM) and with a -DCONSOL_MIN_CTAS=1 build: which occupancy wins.
 
     nvcc ... -DCONSOL_MIN_CTAS=1 -shared -o tools/libkarpsolve_occ1.so kp_api.cu kp_prep.cpp -lcudart   (in karpenter_b200/csrc)
-    python tools/run_c4_occ.py; python tools/run_c4_occ.py tools/libkarpsolve_occ1.so
-
-Measured on B200 (round 1): 4.7-4.9 ms at 2 CTAs / SM (128 registers, a few spills) vs 5.96 ms at 1 CTA / SM (248 registers)."""
+    python tools/run_c4_occ.py; python tools/run_c4_occ.py tools/libkarpsolve_occ1.so"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from karpenter_b200 import _abi, _native, workloads
