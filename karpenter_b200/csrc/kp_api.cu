@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -67,7 +68,7 @@ struct Arena {  // device allocations of one upload, bump-allocated from chunks 
 };
 
 // One uploaded problem == one Scheduler instance (scheduler.go:116-184): its tables in HBM and what the host needs to
-// assemble the result.  A handle owns one for kp_solve / kp_consolidate and a vector of them for kp_solve_batch.
+// assemble the result.  A handle owns one for kp_solve / kp_consolidate and several for kp_solve_batch.
 struct Instance {
   KpDev dev;
   HostTables host;
@@ -85,7 +86,6 @@ struct Instance {
   int32_t *d_nsig_rs = nullptr, *d_nsig_tolset = nullptr;
   int64_t* d_rv_req = nullptr;
   int strict_undefined = 0;
-  float wsolve_ms = 0;
   // state the solve mutates: pristine device copies, restored device-to-device before every solve (no host memory,
   // no allocation and no synchronisation sits between the first and the last kernel of a solve)
   struct Reset {
@@ -158,11 +158,13 @@ struct kp_handle {
   cudaStream_t stream = nullptr;
   std::string err;
   Arena arena;
-  Instance main;
-  std::vector<Instance*> batch;  // kp_upload_batch
-  Instance* cur = &main;          // the instance the helpers below work on
-  KpDev* d_batch_devs = nullptr;  // [batch] device copies of the instances' pointer blocks
-  int2* d_batch_plan = nullptr;   // [batch] {CS, CR}
+  // the instances of the last upload and the entry point that made it: kp_upload (also kp_solve, kp_feasibility and
+  // kp_consolidate) uploads one, kp_upload_batch / kp_solve_batch any number
+  enum Uploader { NONE, SINGLE, BATCH } uploaded = NONE;
+  std::vector<std::unique_ptr<Instance>> insts;
+  KpDev* d_devs = nullptr;  // [devs_cap] device copies of the instances' pointer blocks (run_solve)
+  int2* d_plan = nullptr;   // [devs_cap] {CS, CR}
+  int devs_cap = 0;
   // sharded job: NCCL communicator + the global topology-domain counter table (device resident, all-reduced per solve)
   void* comm = nullptr;
   int comm_rank = 0, comm_world = 1;
@@ -171,7 +173,7 @@ struct kp_handle {
   float allreduce_ms = 0;
   cudaEvent_t ev3 = nullptr;
   kp_stats stats{};
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 };
 
 template <class T>
@@ -186,14 +188,14 @@ static cudaError_t up(kp_handle* h, const T** dst, const std::vector<T>& v) {
 }
 // a table the solve mutates: the upload goes to a pristine copy, the working copy is restored from it per solve
 template <class T>
-static cudaError_t up_mut(kp_handle* h, T** dst, const std::vector<T>& v) {
+static cudaError_t up_mut(kp_handle* h, Instance& in, T** dst, const std::vector<T>& v) {
   const T* init;
   cudaError_t e = up(h, &init, v);
   if (e != cudaSuccess) return e;
   T* work;
   e = h->arena.alloc(&work, v.size());
   if (e != cudaSuccess) return e;
-  if (!v.empty()) h->cur->resets.push_back(Instance::Reset{work, init, v.size() * sizeof(T)});
+  if (!v.empty()) in.resets.push_back(Instance::Reset{work, init, v.size() * sizeof(T)});
   *dst = work;
   return cudaSuccess;
 }
@@ -285,8 +287,6 @@ int kp_debug_slot_algebra(kp_handle* h, const int64_t* value_int, uint64_t value
   cudaFree(dout);
   return KP_OK;
 }
-
-static void batch_clear(kp_handle* h);
 }
 
 extern "C" {
@@ -319,7 +319,6 @@ int kp_create(int device, kp_handle** out) {
   }
   cudaEventCreate(&h->ev0);
   cudaEventCreate(&h->ev1);
-  cudaEventCreate(&h->ev2);
   cudaEventCreate(&h->ev3);
   cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device);
   cudaDeviceSetLimit(cudaLimitStackSize, 16384);  // pdqsort emulation recurses (log n deep)
@@ -331,7 +330,8 @@ void kp_destroy(kp_handle* h) {
   if (!h) return;
   cudaSetDevice(h->device);
   h->arena.destroy();
-  for (Instance* b : h->batch) delete b;
+  cudaFree(h->d_devs);
+  cudaFree(h->d_plan);
   if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
   if (h->ev3) cudaEventDestroy(h->ev3);
   if (h->ev0) cudaEventDestroy(h->ev0);
@@ -347,9 +347,9 @@ int kp_get_stats(kp_handle* h, kp_stats* out) {
   return KP_OK;
 }
 
-static int upload_tables(kp_handle* h, const kp_problem* p, int cmax_hint) {
-  HostTables& t = h->cur->host;
-  KpDev& d = h->cur->dev;
+static int upload_tables(kp_handle* h, Instance& in, const kp_problem* p, int cmax_hint) {
+  HostTables& t = in.host;
+  KpDev& d = in.dev;
   memset(&d, 0, sizeof(d));
   d.K = t.K;
   d.R = t.R;
@@ -387,6 +387,8 @@ static int upload_tables(kp_handle* h, const kp_problem* p, int cmax_hint) {
   CK(up(h, &d.ge_off, t.ge_off));
   CK(up(h, &d.ge_vals, t.ge_vals));
   CK(up(h, &d.ge_bits, t.ge_bits));
+  d.n_ge = (int)t.ge_vals.size();
+  d.n_itv = std::max(t.itv_off[d.K], 1);
   CK(up(h, &d.off_slots, t.off_slots));
   CK(up(h, &d.off_keys, t.off_keys));
   CK(up(h, &d.offset_bits, t.offset_bits));
@@ -396,7 +398,7 @@ static int upload_tables(kp_handle* h, const kp_problem* p, int cmax_hint) {
   CK(up(h, &d.tmpl_its_raw, t.tmpl_its_raw));
   CK(zeros(h, &d.tmpl_its, t.tmpl_its_raw.size()));
   CK(up(h, &d.tmpl_daemon, t.tmpl_daemon));
-  CK(up_mut(h, &d.tmpl_remaining, t.tmpl_remaining));
+  CK(up_mut(h, in, &d.tmpl_remaining, t.tmpl_remaining));
   CK(up(h, &d.tmpl_limit_present, t.tmpl_limit_present));
   CK(up(h, &d.cls_req, t.cls_req));
   CK(up(h, &d.cls_rs, t.cls_rs));
@@ -572,7 +574,7 @@ static int upload_tables(kp_handle* h, const kp_problem* p, int cmax_hint) {
     d.n_fsig = (int)fsigs.size();
     d.n_nsig = (int)nsigs.size();
     d.EW = (t.E + 31) / 32;
-    h->cur->strict_undefined = nodes_gain_keys ? 0 : 1;
+    in.strict_undefined = nodes_gain_keys ? 0 : 1;
     if (hchk.empty()) hchk.push_back(int4{0, 0, 0, 0});
     if (nsig_rs.empty()) {
       nsig_rs.push_back(0);
@@ -587,15 +589,15 @@ static int upload_tables(kp_handle* h, const kp_problem* p, int cmax_hint) {
       CK(up(h, &a_, nsig_rs));
       CK(up(h, &b_, nsig_tolset));
       CK(up(h, &c_, rv_req));
-      h->cur->d_nsig_rs = const_cast<int32_t*>(a_);
-      h->cur->d_nsig_tolset = const_cast<int32_t*>(b_);
-      h->cur->d_rv_req = const_cast<int64_t*>(c_);
+      in.d_nsig_rs = const_cast<int32_t*>(a_);
+      in.d_nsig_tolset = const_cast<int32_t*>(b_);
+      in.d_rv_req = const_cast<int64_t*>(c_);
     }
     CK(up(h, &d.cls_hchk, hchk));
     std::vector<uint32_t> nact(std::max(d.EW, 1), 0);
     for (int n = 0; n < t.E; n++)
       if (t.node_flags[n] & KP_NODE_SCHEDULABLE) nact[n >> 5] |= 1u << (n & 31);
-    CK(up_mut(h, &d.nactive, nact));
+    CK(up_mut(h, in, &d.nactive, nact));
     d.ESW = (d.EW + 31) / 32;
     CK(zeros(h, &d.nfit_sum, (size_t)std::max(t.n_rv, 1) * std::max(d.ESW, 1)));
     CK(zeros(h, &d.nstat_sum, (size_t)std::max(d.n_nsig, 1) * std::max(d.ESW, 1)));
@@ -641,25 +643,25 @@ static int upload_tables(kp_handle* h, const kp_problem* p, int cmax_hint) {
   }
   CK(up(h, &d.groups, t.groups));
   CK(up(h, &d.filter_rs, t.filter_rs));
-  CK(up_mut(h, &d.dom_cnt, t.dom_cnt));
-  CK(up_mut(h, &d.dom_reg, t.dom_reg));
-  CK(up_mut(h, &d.dom_pop, t.dom_pop));
+  CK(up_mut(h, in, &d.dom_cnt, t.dom_cnt));
+  CK(up_mut(h, in, &d.dom_reg, t.dom_reg));
+  CK(up_mut(h, in, &d.dom_pop, t.dom_pop));
   d.n_lazy = 0;
   for (int32_t b : t.g_born) d.n_lazy += b == 0;
-  CK(up_mut(h, &d.g_born, t.g_born));
-  CK(up_mut(h, &d.g_birth, t.g_birth));
+  CK(up_mut(h, in, &d.g_born, t.g_born));
+  CK(up_mut(h, in, &d.g_birth, t.g_birth));
   CK(up(h, &d.cls_lazy_off, t.cls_lazy_off));
   CK(up(h, &d.cls_lazy, t.cls_lazy));
-  CK(up_mut(h, &d.g_ndomains, t.g_ndomains));
-  CK(up_mut(h, &d.g_nempty, t.g_nempty));
+  CK(up_mut(h, in, &d.g_ndomains, t.g_ndomains));
+  CK(up_mut(h, in, &d.g_nempty, t.g_nempty));
   CK(up(h, &d.node_taintset, t.node_taintset));
   CK(up(h, &d.node_flags, t.node_flags));
-  CK(up_mut(h, &d.node_rem, t.node_rem));
-  CK(up_mut(h, &d.node_rem_present, t.node_rem_present));
-  CK(up_mut(h, &d.node_sflags, t.node_sflags));
-  CK(up_mut(h, &d.node_smask, t.node_smask));
-  CK(up_mut(h, &d.node_sgte, t.node_sgte));
-  CK(up_mut(h, &d.node_slte, t.node_slte));
+  CK(up_mut(h, in, &d.node_rem, t.node_rem));
+  CK(up_mut(h, in, &d.node_rem_present, t.node_rem_present));
+  CK(up_mut(h, in, &d.node_sflags, t.node_sflags));
+  CK(up_mut(h, in, &d.node_smask, t.node_smask));
+  CK(up_mut(h, in, &d.node_sgte, t.node_sgte));
+  CK(up_mut(h, in, &d.node_slte, t.node_slte));
   CK(zeros(h, &d.node_npods, (size_t)std::max(t.E, 1)));
   // claims
   d.Cmax = cmax_hint;
@@ -688,7 +690,7 @@ static int upload_tables(kp_handle* h, const kp_problem* p, int cmax_hint) {
       if (d.n_hostports && p->node_hostports) np[n] = p->node_hostports[n];
     for (int n = 0; n < t.N; n++)
       if (d.n_hostports && p->tmpl_hostports) tp[n] = p->tmpl_hostports[n];
-    CK(up_mut(h, &d.node_ports, np));
+    CK(up_mut(h, in, &d.node_ports, np));
     CK(up(h, &d.tmpl_ports, tp));
     CK(zeros(h, &d.c_ports, C));
   }
@@ -705,7 +707,7 @@ static int upload_tables(kp_handle* h, const kp_problem* p, int cmax_hint) {
     CK(up(h, &d.set_rsv, sr));
     std::vector<int32_t> cap0 = t.rsv_cap0;
     if (cap0.empty()) cap0.push_back(0);
-    CK(up_mut(h, &d.rsv_cap, cap0));
+    CK(up_mut(h, in, &d.rsv_cap, cap0));
     CK(zeros(h, &d.c_rsv, C));
     d.rsv_ct_key = p->reservation_capacity_type_key;
     d.rsv_reserved_val = p->reservation_reserved_value;
@@ -729,7 +731,7 @@ static int upload_tables(kp_handle* h, const kp_problem* p, int cmax_hint) {
     std::vector<int32_t> tr((size_t)std::max(t.E, 1) * d.GHS, 0);
     for (int r = 0; r < t.GH; r++)
       for (int n = 0; n < t.E; n++) tr[(size_t)n * d.GHS + r] = t.host_cnt_nodes[(size_t)r * t.E + n];
-    CK(up(h, &h->cur->d_host_cnt_nodes, tr));
+    CK(up(h, &in.d_host_cnt_nodes, tr));
   }
   d.HW = (d.H + 31) / 32;
   CK(zeros(h, &d.host_pop, (size_t)std::max(t.GH, 1) * d.HW));
@@ -739,7 +741,7 @@ static int upload_tables(kp_handle* h, const kp_problem* p, int cmax_hint) {
     for (int r = 0; r < t.GH; r++)
       for (int n = 0; n < t.E; n++)
         if (t.host_cnt_nodes[(size_t)r * t.E + n] > 0) bits[(size_t)r * ew + (n >> 5)] |= 1u << (n & 31);
-    CK(up(h, &h->cur->d_host_pop_nodes, bits));
+    CK(up(h, &in.d_host_pop_nodes, bits));
   }
   CK(zeros(h, &d.n_claims, 1));
   CK(zeros(h, &d.counters, 16));
@@ -748,252 +750,75 @@ static int upload_tables(kp_handle* h, const kp_problem* p, int cmax_hint) {
 }
 
 // stack of state the solve mutates, so kp_solve_resident can be re-run on the same upload
-static int reset_dynamic(kp_handle* h) {
-  HostTables& t = h->cur->host;
-  KpDev& d = h->cur->dev;
-  for (auto& r : h->cur->resets) CK(cudaMemcpyAsync(r.dst, r.src, r.bytes, cudaMemcpyDeviceToDevice, h->stream));
+static int reset_dynamic(kp_handle* h, Instance& in) {
+  HostTables& t = in.host;
+  KpDev& d = in.dev;
+  for (auto& r : in.resets) CK(cudaMemcpyAsync(r.dst, r.src, r.bytes, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemsetAsync(d.node_npods, 0, (size_t)std::max(t.E, 1) * 4, h->stream));
   size_t C = (size_t)d.Cmax;
   CK(cudaMemsetAsync(d.c_npods, 0, C * 4, h->stream));
   CK(cudaMemsetAsync(d.cmask, 0, C * sizeof(ulonglong2), h->stream));
   CK(cudaMemsetAsync(d.amask, 0, C * 8, h->stream));
   CK(cudaMemsetAsync(d.c_rsv, 0, C * 8, h->stream));
-  if (h->cur->d_dropped) CK(cudaMemsetAsync(h->cur->d_dropped, 0, C, h->stream));
+  if (in.d_dropped) CK(cudaMemsetAsync(in.d_dropped, 0, C, h->stream));
   CK(cudaMemsetAsync(d.host_cnt, 0, (size_t)d.GHS * d.H * 4, h->stream));
   if (t.E && t.GH)  // initial hostname-group counts of the existing nodes: the first E host rows
-    CK(cudaMemcpyAsync(d.host_cnt, h->cur->d_host_cnt_nodes, (size_t)t.E * d.GHS * 4, cudaMemcpyDeviceToDevice, h->stream));
+    CK(cudaMemcpyAsync(d.host_cnt, in.d_host_cnt_nodes, (size_t)t.E * d.GHS * 4, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemsetAsync(d.host_pop, 0, (size_t)std::max(t.GH, 1) * d.HW * 4, h->stream));
   if (t.E && t.GH) {
     const size_t ew = (size_t)(t.E + 31) / 32;
-    CK(cudaMemcpy2DAsync(d.host_pop, (size_t)d.HW * 4, h->cur->d_host_pop_nodes, ew * 4, ew * 4, t.GH,
+    CK(cudaMemcpy2DAsync(d.host_pop, (size_t)d.HW * 4, in.d_host_pop_nodes, ew * 4, ew * 4, t.GH,
                          cudaMemcpyDeviceToDevice, h->stream));
   }
   CK(cudaMemsetAsync(d.n_claims, 0, 4, h->stream));
   CK(cudaMemsetAsync(d.counters, 0, 128, h->stream));
   CK(cudaMemsetAsync(d.status, 0, 4, h->stream));
-  CK(cudaMemsetAsync(d.last_len, 0, (size_t)std::max<int64_t>(h->cur->P, 1) * 4, h->stream));
+  CK(cudaMemsetAsync(d.last_len, 0, (size_t)std::max<int64_t>(in.P, 1) * 4, h->stream));
   return KP_OK;
 }
 
-static int do_upload(kp_handle* h, const kp_problem* p, int cmax, bool fresh_arena = true) {
-  cudaSetDevice(h->device);
-  cudaStreamSynchronize(h->stream);
-  if (fresh_arena) {
-    if (h->cur == &h->main) batch_clear(h);  // the arena is shared: a fresh single upload invalidates every batch instance
-    h->main.resident = false;
-    h->d_gcnt = nullptr;  // lived in the arena
-    h->gcnt_slots = 0;
-    h->arena.reset();
-  }
-  h->cur->resets.clear();
-  h->cur->resident = false;
-  h->stats = kp_stats{};
-  auto t0 = std::chrono::steady_clock::now();
-  h->cur->host = HostTables();
-  std::vector<uint8_t> active(p->n_nodes, 0);
-  for (int i = 0; i < p->n_nodes; i++) active[i] = (p->node_flags[i] & KP_NODE_SCHEDULABLE) != 0;
-  std::vector<int32_t> pending(p->pod_class, p->pod_class + p->n_pods);
-  int rc = kp_prepare(p, active, {}, pending, h->cur->host, h->err);
-  if (rc != KP_OK) return rc;
-  auto t1 = std::chrono::steady_clock::now();
-  h->stats.prep_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
-  h->cur->P = p->n_pods;
-  h->cur->n_keys = p->n_keys;
-  h->cur->n_resources = p->n_resources;
-  h->cur->n_its = p->n_its;
-  h->cur->n_nodes = p->n_nodes;
-  h->cur->hostname_key = h->cur->host.hostname_key;
-  h->cur->key_nvalues.resize(p->n_keys);
-  for (int k = 0; k < p->n_keys; k++) h->cur->key_nvalues[k] = p->key_value_off[k + 1] - p->key_value_off[k];
-  if (p->n_pods >= (1ll << 31) - 2) return h->err = "more than 2^31 pods", KP_ERR_CAPACITY;
-  rc = upload_tables(h, p, cmax);
-  if (rc != KP_OK) return rc;
-  KpDev& d = h->cur->dev;
-  d.P = p->n_pods;
-  size_t P = (size_t)p->n_pods;
-  CK(up_raw(h, &h->cur->d_pod_class, p->pod_class, P));
-  d.pod_class = h->cur->d_pod_class;
-  if (p->pod_creation) {
-    CK(up_raw(h, &h->cur->d_pod_creation, p->pod_creation, P));
-  } else {
-    CK(zeros(h, &h->cur->d_pod_creation, P));
-  }
-  CK(up_raw(h, &h->cur->d_uid_hi, p->pod_uid_hi, P));
-  CK(up_raw(h, &h->cur->d_uid_lo, p->pod_uid_lo, P));
-  // class rank for byCPUAndMemoryDescending (queue.go:72-108): cpu desc, then memory desc
-  std::vector<int64_t> rank(std::max(h->cur->host.X, 1), 0);
-  {
-    std::vector<int> idx(h->cur->host.X);
-    for (int i = 0; i < h->cur->host.X; i++) idx[i] = i;
-    auto key = [&](int x) { return std::make_pair(-h->cur->host.cls_sort_cpu[x], -h->cur->host.cls_sort_mem[x]); };
-    std::sort(idx.begin(), idx.end(), [&](int a, int b) { return key(a) < key(b); });
-    int64_t r = -1;
-    for (size_t i = 0; i < idx.size(); i++) {
-      if (i == 0 || key(idx[i]) != key(idx[i - 1])) r++;
-      rank[idx[i]] = r;
+// OrderByPrice lists: available offerings per instance type, cheapest first (types.go:238-257)
+struct PriceLists {
+  std::vector<int32_t> off, set;
+  std::vector<double> price;
+};
+static PriceLists order_by_price(const kp_problem* p, const HostTables& t) {
+  PriceLists l;
+  l.off.assign((size_t)p->n_its + 1, 0);
+  for (int ti = 0; ti < p->n_its; ti++) {
+    std::vector<std::pair<double, int>> ent;
+    for (int o = p->it_off_off[ti]; o < p->it_off_off[ti + 1]; o++)
+      if (p->off_available[o]) ent.push_back({p->off_price[o], t.off_set[o]});
+    std::stable_sort(ent.begin(), ent.end(),
+                     [](const std::pair<double, int>& a, const std::pair<double, int>& b) { return a.first < b.first; });
+    for (auto& e : ent) {
+      l.price.push_back(e.first);
+      l.set.push_back(e.second);
     }
+    l.off[(size_t)ti + 1] = (int32_t)l.set.size();
   }
-  CK(up_raw(h, &h->cur->d_class_rank, rank.data(), rank.size()));
-  {
-    // Pods of classes that are alone in their (cpu, memory) rank stand together in the queue (byCPUAndMemoryDescending, then
-    // creation time and UID, which interleave the classes of one rank): when they are at least a quarter of the queue the
-    // solve runs the cohort instantiation.  KP_COHORT=1 / KP_NO_COHORT=1 force the choice.
-    const int X = h->cur->host.X;
-    std::vector<int64_t> pods_of(std::max(X, 1), 0), classes_at(std::max(X, 1), 0);
-    for (size_t i = 0; i < P; i++) pods_of[p->pod_class[i]]++;
-    for (int x = 0; x < X; x++)
-      if (pods_of[x] > 0) classes_at[rank[x]]++;
-    int64_t in_runs = 0;
-    for (int x = 0; x < X; x++)
-      if (pods_of[x] > 1 && classes_at[rank[x]] == 1) in_runs += pods_of[x];
-    h->cur->cohort = (in_runs * 4 >= (int64_t)P && P > 0 && !getenv("KP_NO_COHORT")) || getenv("KP_COHORT");
-    d.cohort = h->cur->cohort ? 1 : 0;
+  if (l.set.empty()) {
+    l.set.push_back(0);
+    l.price.push_back(0);
   }
-  h->cur->max_its = p->max_instance_types > 0 ? p->max_instance_types : 0;
-  if (h->cur->max_its > 0) {
-    const HostTables& t = h->cur->host;
-    const int T = p->n_its;
-    // OrderByPrice lists: available offerings per instance type, cheapest first (types.go:238-257)
-    std::vector<int32_t> ml_off((size_t)T + 1, 0), ml_set;
-    std::vector<double> ml_price;
-    for (int ti = 0; ti < T; ti++) {
-      std::vector<std::pair<double, int>> ent;
-      for (int o = p->it_off_off[ti]; o < p->it_off_off[ti + 1]; o++)
-        if (p->off_available[o]) ent.push_back({p->off_price[o], t.off_set[o]});
-      std::stable_sort(ent.begin(), ent.end(),
-                       [](const std::pair<double, int>& a, const std::pair<double, int>& b) { return a.first < b.first; });
-      for (auto& e : ent) {
-        ml_price.push_back(e.first);
-        ml_set.push_back(e.second);
-      }
-      ml_off[(size_t)ti + 1] = (int32_t)ml_set.size();
-    }
-    if (ml_set.empty()) {
-      ml_set.push_back(0);
-      ml_price.push_back(0);
-    }
-    CK(up(h, &h->cur->price_tabs.ml_off, ml_off));
-    CK(up(h, &h->cur->price_tabs.ml_set, ml_set));
-    CK(up(h, &h->cur->price_tabs.ml_price, ml_price));
-    const size_t NW = (size_t)KP_TRUNC_BLOCKS * 4;
-    CK(h->arena.alloc(&h->cur->trunc_key, NW * std::max(T, 1)));
-    CK(h->arena.alloc(&h->cur->trunc_val, NW * std::max(T, 1)));
-    CK(h->arena.alloc(&h->cur->trunc_bits, NW * std::max((T + 63) / 64, 1)));
-    CK(zeros(h, &h->cur->d_dropped, (size_t)std::max<int64_t>(h->cur->dev.Cmax, 1)));
-  }
-  {  // NewQueue sort: key / permutation ping-pong buffers and cub's scratch, sized once per upload
-    int64_t* ka;
-    int64_t* kb;
-    CK(h->arena.alloc(&ka, P));
-    CK(h->arena.alloc(&kb, P));
-    CK(h->arena.alloc(&h->cur->sort_perm_b, P));
-    h->cur->sort_keys_a = ka;
-    h->cur->sort_keys_b = kb;
-    size_t n1 = 0, n2 = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, n1, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const int32_t*)nullptr,
-                                    (int32_t*)nullptr, (int)std::max<size_t>(P, 1));
-    cub::DeviceRadixSort::SortPairs(nullptr, n2, (const int64_t*)nullptr, (int64_t*)nullptr, (const int32_t*)nullptr,
-                                    (int32_t*)nullptr, (int)std::max<size_t>(P, 1));
-    h->cur->sort_tmp_bytes = std::max(n1, n2);
-    char* tmp;
-    CK(h->arena.alloc(&tmp, h->cur->sort_tmp_bytes));
-    h->cur->sort_tmp = tmp;
-  }
-  CK(zeros(h, &d.queue, P + 1));
-  CK(zeros(h, &d.qcls, P + 1));
-  CK(zeros(h, &d.last_len, P));
-  CK(zeros(h, &d.pod_target, P));
-  CK(zeros(h, &d.pod_error, P));
-  CK(cudaStreamSynchronize(h->stream));
-  auto t2 = std::chrono::steady_clock::now();
-  h->stats.upload_ms = std::chrono::duration<double, std::milli>(t2 - t1).count();
-  h->cur->resident = true;
-  return KP_OK;
+  return l;
 }
 
-int kp_upload(kp_handle* h, const kp_problem* p) {
-  // claim capacity: every pod could need its own NodeClaim; start with a generous bound and grow on demand
-  int64_t guess = std::min<int64_t>(p->n_pods, std::max<int64_t>(4096, p->n_pods / 8));
-  return do_upload(h, p, (int)std::max<int64_t>(guess, 1));
+// shared-memory bytes of the read-only tables a kernel stages next to `fixed` bytes of its own (0 = leave them in L2)
+static int plan_tables(const KpDev& d, size_t fixed, size_t budget) {
+  const size_t tb = kp_tab_bytes(d);
+  return (fixed + tb <= budget && tb <= 110 * 1024) ? (int)tb : 0;
 }
 
-// NewQueue: sort pods cpu desc, mem desc, creation asc, uid asc (queue.go:37-43) into d.queue / d.qcls.
-// Four LSD passes of a stable radix sort (cub), each on a gathered 64-bit key.
-__global__ void k_iota(int32_t* p, int64_t n) {
-  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i < n) p[i] = (int32_t)i;
-}
-
-static int sort_queue(kp_handle* h) {
-  KpDev& d = h->cur->dev;
-  const int64_t P = h->cur->P;
-  if (P <= 0) return KP_OK;
-  const int nb = (int)((P + 255) / 256), n = (int)P;
-  int32_t* perm_a = d.queue;  // passes ping-pong a -> b -> a -> b -> a: the result lands in d.queue
-  int32_t* perm_b = h->cur->sort_perm_b;
-  uint64_t *ua = (uint64_t*)h->cur->sort_keys_a, *ub = (uint64_t*)h->cur->sort_keys_b;
-  int64_t *sa = (int64_t*)h->cur->sort_keys_a, *sb = (int64_t*)h->cur->sort_keys_b;
-  size_t tb = h->cur->sort_tmp_bytes;
-  k_iota<<<nb, 256, 0, h->stream>>>(perm_a, P);
-  k_gather<<<nb, 256, 0, h->stream>>>(h->cur->d_uid_lo, perm_a, P, ua);
-  CK(cub::DeviceRadixSort::SortPairs(h->cur->sort_tmp, tb, ua, ub, perm_a, perm_b, n, 0, 64, h->stream));
-  k_gather<<<nb, 256, 0, h->stream>>>(h->cur->d_uid_hi, perm_b, P, ua);
-  CK(cub::DeviceRadixSort::SortPairs(h->cur->sort_tmp, tb, ua, ub, perm_b, perm_a, n, 0, 64, h->stream));
-  k_gather<<<nb, 256, 0, h->stream>>>(h->cur->d_pod_creation, perm_a, P, sa);
-  CK(cub::DeviceRadixSort::SortPairs(h->cur->sort_tmp, tb, sa, sb, perm_a, perm_b, n, 0, 64, h->stream));
-  k_sort_keys<<<nb, 256, 0, h->stream>>>(d.pod_class, h->cur->d_class_rank, perm_b, P, sa);
-  CK(cub::DeviceRadixSort::SortPairs(h->cur->sort_tmp, tb, sa, sb, perm_b, perm_a, n, 0, 64, h->stream));
-  k_gather<<<nb, 256, 0, h->stream>>>(d.pod_class, d.queue, P, d.qcls);
-  h->stats.kernel_launches += 6;
-  return KP_OK;
-}
-
-// shared-memory plan of a kernel that stages the read-only tables: returns the table bytes to stage (0 = leave in L2)
-static size_t plan_tables(kp_handle* h, size_t fixed, size_t budget) {
-  KpDev& d = h->cur->dev;
-  d.n_ge = (int)h->cur->host.ge_vals.size();
-  d.n_itv = std::max(h->cur->host.itv_off[d.K], 1);
-  size_t tb = kp_tab_bytes(d);
-  d.tab_bytes = (fixed + tb <= budget && tb <= 110 * 1024) ? (int)tb : 0;
-  return (size_t)d.tab_bytes;
-}
-
-static int launch_node_cand(kp_handle* h) {
-  KpDev& d = h->cur->dev;
-  if (d.E <= 0) return KP_OK;
-  dim3 grid((d.E + 255) / 256, d.n_nsig + d.n_rv);
-  k_node_cand<<<grid, 256, 0, h->stream>>>(d, h->cur->d_nsig_rs, h->cur->d_nsig_tolset, h->cur->d_rv_req, h->cur->strict_undefined);
-  const int nsum = (d.n_rv + d.n_nsig) * d.ESW;
-  k_node_sum<<<(nsum + 255) / 256, 256, 0, h->stream>>>(d);
-  h->stats.kernel_launches += 2;
-  return KP_OK;
-}
-
-// Everything of a solve in front of the solver kernel (after reset_dynamic): NewScheduler prefilter, NewQueue,
-// existing-node candidate bitmaps, and the shared-memory plan of the solver CTA.  Asynchronous on the handle's stream.
-static int prep_solve(kp_handle* h) {
-  Instance& in = *h->cur;
+// Host-side plan of the solver CTA; it depends on the upload and the KP_* knobs only.  Shared memory holds the pointer
+// block, the staged tables and, when they fit, the rows of the first CR claims and the claim order, template ids and
+// failure bitmaps of the first CS claims.
+static void plan_solve(Instance& in) {
   KpDev& d = in.dev;
-  int rc;
-  int64_t P = in.P;
-  // NewScheduler prefilter of template instance types (scheduler.go:147)
-  if (d.N > 0) {
-    k_feasibility<<<(d.N * 32 + 255) / 256, 256, 0, h->stream>>>(d, nullptr, 1);
-    h->stats.kernel_launches++;
-  }
-  rc = sort_queue(h);
-  if (rc != KP_OK) return rc;
-  if (P > 0) {
-    k_fill_i32<<<(int)((P + 255) / 256), 256, 0, h->stream>>>(d.pod_target, P, KP_TARGET_UNSCHEDULED);
-    h->stats.kernel_launches++;
-  }
-  rc = launch_node_cand(h);
-  if (rc != KP_OK) return rc;
-  // shared memory of the solve CTA: pointer block + staged tables + (when they fit) claim order, template ids and
-  // the failure bitmaps
   const size_t budget = 224 * 1024;
   const size_t fixed = KP_ALIGN16(sizeof(WSolveShared));
-  size_t tb = plan_tables(h, fixed, budget);
+  d.tab_bytes = plan_tables(d, fixed, budget);
+  size_t tb = d.tab_bytes;
   // rows of the first CR claims (requirement slots, requests, threshold rows, instance-type words) ...
   auto row_bytes = [&](int cr) {
     return KP_ALIGN16((size_t)cr * d.K * 8) + KP_ALIGN16((size_t)cr * d.R * 8) + KP_ALIGN16((size_t)cr * d.ITW * 8) +
@@ -1028,20 +853,218 @@ static int prep_solve(kp_handle* h) {
   in.CS = CS;
   in.CR = CR;
   in.smem = fixed + tb + (CS ? small_bytes(CS) : 0) + 64;
+}
+
+// Starts a fresh upload: the instances of either entry point are dropped and the arena is reused for the new ones.
+static void begin_upload(kp_handle* h, kp_handle::Uploader by) {
+  cudaSetDevice(h->device);
+  cudaStreamSynchronize(h->stream);
+  h->insts.clear();
+  h->uploaded = by;
+  h->d_gcnt = nullptr;  // lived in the arena
+  h->gcnt_slots = 0;
+  h->arena.reset();
+  h->stats = kp_stats{};
+}
+
+// Uploads p as one more instance of the handle, room for `cmax` NodeClaims.  The stats sum over the instances.
+static int add_instance(kp_handle* h, const kp_problem* p, int64_t cmax) {
+  h->insts.push_back(std::make_unique<Instance>());
+  Instance& in = *h->insts.back();
+  auto t0 = std::chrono::steady_clock::now();
+  std::vector<uint8_t> active(p->n_nodes, 0);
+  for (int i = 0; i < p->n_nodes; i++) active[i] = (p->node_flags[i] & KP_NODE_SCHEDULABLE) != 0;
+  std::vector<int32_t> pending(p->pod_class, p->pod_class + p->n_pods);
+  int rc = kp_prepare(p, active, {}, pending, in.host, h->err);
+  if (rc != KP_OK) return rc;
+  auto t1 = std::chrono::steady_clock::now();
+  h->stats.prep_ms += std::chrono::duration<double, std::milli>(t1 - t0).count();
+  in.P = p->n_pods;
+  in.n_keys = p->n_keys;
+  in.n_resources = p->n_resources;
+  in.n_its = p->n_its;
+  in.n_nodes = p->n_nodes;
+  in.hostname_key = in.host.hostname_key;
+  in.key_nvalues.resize(p->n_keys);
+  for (int k = 0; k < p->n_keys; k++) in.key_nvalues[k] = p->key_value_off[k + 1] - p->key_value_off[k];
+  if (p->n_pods >= (1ll << 31) - 2) return h->err = "more than 2^31 pods", KP_ERR_CAPACITY;
+  rc = upload_tables(h, in, p, (int)cmax);
+  if (rc != KP_OK) return rc;
+  KpDev& d = in.dev;
+  d.P = p->n_pods;
+  size_t P = (size_t)p->n_pods;
+  CK(up_raw(h, &in.d_pod_class, p->pod_class, P));
+  d.pod_class = in.d_pod_class;
+  if (p->pod_creation) {
+    CK(up_raw(h, &in.d_pod_creation, p->pod_creation, P));
+  } else {
+    CK(zeros(h, &in.d_pod_creation, P));
+  }
+  CK(up_raw(h, &in.d_uid_hi, p->pod_uid_hi, P));
+  CK(up_raw(h, &in.d_uid_lo, p->pod_uid_lo, P));
+  // class rank for byCPUAndMemoryDescending (queue.go:72-108): cpu desc, then memory desc
+  std::vector<int64_t> rank(std::max(in.host.X, 1), 0);
+  {
+    std::vector<int> idx(in.host.X);
+    for (int i = 0; i < in.host.X; i++) idx[i] = i;
+    auto key = [&](int x) { return std::make_pair(-in.host.cls_sort_cpu[x], -in.host.cls_sort_mem[x]); };
+    std::sort(idx.begin(), idx.end(), [&](int a, int b) { return key(a) < key(b); });
+    int64_t r = -1;
+    for (size_t i = 0; i < idx.size(); i++) {
+      if (i == 0 || key(idx[i]) != key(idx[i - 1])) r++;
+      rank[idx[i]] = r;
+    }
+  }
+  CK(up_raw(h, &in.d_class_rank, rank.data(), rank.size()));
+  {
+    // Pods of classes that are alone in their (cpu, memory) rank stand together in the queue (byCPUAndMemoryDescending, then
+    // creation time and UID, which interleave the classes of one rank): when they are at least a quarter of the queue the
+    // solve runs the cohort instantiation.  KP_COHORT=1 / KP_NO_COHORT=1 force the choice.
+    const int X = in.host.X;
+    std::vector<int64_t> pods_of(std::max(X, 1), 0), classes_at(std::max(X, 1), 0);
+    for (size_t i = 0; i < P; i++) pods_of[p->pod_class[i]]++;
+    for (int x = 0; x < X; x++)
+      if (pods_of[x] > 0) classes_at[rank[x]]++;
+    int64_t in_runs = 0;
+    for (int x = 0; x < X; x++)
+      if (pods_of[x] > 1 && classes_at[rank[x]] == 1) in_runs += pods_of[x];
+    in.cohort = (in_runs * 4 >= (int64_t)P && P > 0 && !getenv("KP_NO_COHORT")) || getenv("KP_COHORT");
+    d.cohort = in.cohort ? 1 : 0;
+  }
+  in.max_its = p->max_instance_types > 0 ? p->max_instance_types : 0;
+  if (in.max_its > 0) {
+    const int T = p->n_its;
+    const PriceLists ml = order_by_price(p, in.host);
+    CK(up(h, &in.price_tabs.ml_off, ml.off));
+    CK(up(h, &in.price_tabs.ml_set, ml.set));
+    CK(up(h, &in.price_tabs.ml_price, ml.price));
+    const size_t NW = (size_t)KP_TRUNC_BLOCKS * 4;
+    CK(h->arena.alloc(&in.trunc_key, NW * std::max(T, 1)));
+    CK(h->arena.alloc(&in.trunc_val, NW * std::max(T, 1)));
+    CK(h->arena.alloc(&in.trunc_bits, NW * std::max((T + 63) / 64, 1)));
+    CK(zeros(h, &in.d_dropped, (size_t)std::max<int64_t>(d.Cmax, 1)));
+  }
+  {  // NewQueue sort: key / permutation ping-pong buffers and cub's scratch, sized once per upload
+    int64_t* ka;
+    int64_t* kb;
+    CK(h->arena.alloc(&ka, P));
+    CK(h->arena.alloc(&kb, P));
+    CK(h->arena.alloc(&in.sort_perm_b, P));
+    in.sort_keys_a = ka;
+    in.sort_keys_b = kb;
+    size_t n1 = 0, n2 = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, n1, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const int32_t*)nullptr,
+                                    (int32_t*)nullptr, (int)std::max<size_t>(P, 1));
+    cub::DeviceRadixSort::SortPairs(nullptr, n2, (const int64_t*)nullptr, (int64_t*)nullptr, (const int32_t*)nullptr,
+                                    (int32_t*)nullptr, (int)std::max<size_t>(P, 1));
+    in.sort_tmp_bytes = std::max(n1, n2);
+    char* tmp;
+    CK(h->arena.alloc(&tmp, in.sort_tmp_bytes));
+    in.sort_tmp = tmp;
+  }
+  CK(zeros(h, &d.queue, P + 1));
+  CK(zeros(h, &d.qcls, P + 1));
+  CK(zeros(h, &d.last_len, P));
+  CK(zeros(h, &d.pod_target, P));
+  CK(zeros(h, &d.pod_error, P));
+  CK(cudaStreamSynchronize(h->stream));
+  auto t2 = std::chrono::steady_clock::now();
+  h->stats.upload_ms += std::chrono::duration<double, std::milli>(t2 - t1).count();
+  plan_solve(in);
+  in.resident = true;
   return KP_OK;
+}
+
+static int upload(kp_handle* h, const kp_problem* const* problems, int n, const int64_t* cmax, kp_handle::Uploader by) {
+  begin_upload(h, by);
+  for (int b = 0; b < n; b++) {
+    int rc = add_instance(h, problems[b], cmax[b]);
+    if (rc != KP_OK) return rc;
+  }
+  return KP_OK;
+}
+
+// claim capacity: every pod could need its own NodeClaim; start with a generous bound and grow on demand
+static int64_t cmax_guess(const kp_problem* p) {
+  return std::max<int64_t>(1, std::min<int64_t>(p->n_pods, std::max<int64_t>(4096, p->n_pods / 8)));
+}
+
+int kp_upload(kp_handle* h, const kp_problem* p) {
+  const int64_t cmax = cmax_guess(p);
+  return upload(h, &p, 1, &cmax, kp_handle::SINGLE);
+}
+
+// NewQueue: sort pods cpu desc, mem desc, creation asc, uid asc (queue.go:37-43) into d.queue / d.qcls.
+// Four LSD passes of a stable radix sort (cub), each on a gathered 64-bit key.
+__global__ void k_iota(int32_t* p, int64_t n) {
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < n) p[i] = (int32_t)i;
+}
+
+static int sort_queue(kp_handle* h, Instance& in) {
+  KpDev& d = in.dev;
+  const int64_t P = in.P;
+  if (P <= 0) return KP_OK;
+  const int nb = (int)((P + 255) / 256), n = (int)P;
+  int32_t* perm_a = d.queue;  // passes ping-pong a -> b -> a -> b -> a: the result lands in d.queue
+  int32_t* perm_b = in.sort_perm_b;
+  uint64_t *ua = (uint64_t*)in.sort_keys_a, *ub = (uint64_t*)in.sort_keys_b;
+  int64_t *sa = (int64_t*)in.sort_keys_a, *sb = (int64_t*)in.sort_keys_b;
+  size_t tb = in.sort_tmp_bytes;
+  k_iota<<<nb, 256, 0, h->stream>>>(perm_a, P);
+  k_gather<<<nb, 256, 0, h->stream>>>(in.d_uid_lo, perm_a, P, ua);
+  CK(cub::DeviceRadixSort::SortPairs(in.sort_tmp, tb, ua, ub, perm_a, perm_b, n, 0, 64, h->stream));
+  k_gather<<<nb, 256, 0, h->stream>>>(in.d_uid_hi, perm_b, P, ua);
+  CK(cub::DeviceRadixSort::SortPairs(in.sort_tmp, tb, ua, ub, perm_b, perm_a, n, 0, 64, h->stream));
+  k_gather<<<nb, 256, 0, h->stream>>>(in.d_pod_creation, perm_a, P, sa);
+  CK(cub::DeviceRadixSort::SortPairs(in.sort_tmp, tb, sa, sb, perm_a, perm_b, n, 0, 64, h->stream));
+  k_sort_keys<<<nb, 256, 0, h->stream>>>(d.pod_class, in.d_class_rank, perm_b, P, sa);
+  CK(cub::DeviceRadixSort::SortPairs(in.sort_tmp, tb, sa, sb, perm_b, perm_a, n, 0, 64, h->stream));
+  k_gather<<<nb, 256, 0, h->stream>>>(d.pod_class, d.queue, P, d.qcls);
+  h->stats.kernel_launches += 6;
+  return KP_OK;
+}
+
+static int launch_node_cand(kp_handle* h, Instance& in) {
+  KpDev& d = in.dev;
+  if (d.E <= 0) return KP_OK;
+  dim3 grid((d.E + 255) / 256, d.n_nsig + d.n_rv);
+  k_node_cand<<<grid, 256, 0, h->stream>>>(d, in.d_nsig_rs, in.d_nsig_tolset, in.d_rv_req, in.strict_undefined);
+  const int nsum = (d.n_rv + d.n_nsig) * d.ESW;
+  k_node_sum<<<(nsum + 255) / 256, 256, 0, h->stream>>>(d);
+  h->stats.kernel_launches += 2;
+  return KP_OK;
+}
+
+// Everything of a solve in front of the solver kernel (after reset_dynamic): NewScheduler prefilter, NewQueue and the
+// existing-node candidate bitmaps.  Asynchronous on the handle's stream.
+static int prep_solve(kp_handle* h, Instance& in) {
+  KpDev& d = in.dev;
+  // NewScheduler prefilter of template instance types (scheduler.go:147)
+  if (d.N > 0) {
+    k_feasibility<<<(d.N * 32 + 255) / 256, 256, 0, h->stream>>>(d, nullptr, 1);
+    h->stats.kernel_launches++;
+  }
+  int rc = sort_queue(h, in);
+  if (rc != KP_OK) return rc;
+  if (in.P > 0) {
+    k_fill_i32<<<(int)((in.P + 255) / 256), 256, 0, h->stream>>>(d.pod_target, in.P, KP_TARGET_UNSCHEDULED);
+    h->stats.kernel_launches++;
+  }
+  return launch_node_cand(h, in);
 }
 
 // The one collective of a NodePool-sharded job (SURVEY.md section 8(e)): every instance of this handle writes the
 // counters of its topology groups into its slice of the global table, then one ncclAllReduce(sum, int32) over NVLink on
 // the library's stream -- device resident from the solver kernel to the reduced table, inside the solve's event window.
-static int reduce_counters(kp_handle* h, const std::vector<Instance*>& insts) {
+static int reduce_counters(kp_handle* h) {
   if (!h->d_gcnt) return KP_OK;
   CK(cudaEventRecord(h->ev3, h->stream));
   CK(cudaMemsetAsync(h->d_gcnt, 0, (size_t)h->gcnt_slots * 4, h->stream));
-  for (Instance* in : insts)
+  for (auto& in : h->insts)
     if (in->n_slots > 0) {
       k_scatter_counts<<<(int)((in->n_slots + 255) / 256), 256, 0, h->stream>>>(in->dev.dom_cnt, in->d_slot_src, in->n_slots,
-                                                                                h->d_gcnt + in->slot_off);
+                                                                                 h->d_gcnt + in->slot_off);
       h->stats.kernel_launches++;
     }
   if (h->comm) {
@@ -1051,49 +1074,118 @@ static int reduce_counters(kp_handle* h, const std::vector<Instance*>& insts) {
   return KP_OK;
 }
 
-static int run_solve(kp_handle* h) {
-  Instance& in = *h->cur;
-  KpDev& d = in.dev;
+// The solver instantiation of a launch: LEAN when every instance is lean, COHORT when any instance wants it, the
+// volume-alternative one when any instance has a chain
+static const void* solver_kernel(const std::vector<std::unique_ptr<Instance>>& insts) {
+  bool lean = true, cohort = false, vol = false;
+  for (auto& in : insts) {
+    lean = lean && in->lean;
+    cohort = cohort || in->cohort;
+    vol = vol || in->host.has_vol_alts;
+  }
+  if (vol) return (const void*)k_wsolve_batch<false, false, true>;
+  return lean ? (cohort ? (const void*)k_wsolve_batch<true, true> : (const void*)k_wsolve_batch<true, false>)
+              : (cohort ? (const void*)k_wsolve_batch<false, true> : (const void*)k_wsolve_batch<false, false>);
+}
+
+// Scheduler.Solve of every uploaded instance, a single solve being a batch of one.  In front of the timed window: the
+// dynamic state is restored and the pointer blocks and {CS, CR} plans are written to the device.  In it: the prep
+// kernels per instance, ONE solver launch (one CTA per instance), truncation and the counter all-reduce.
+// statuses[b]: KP_OK / KP_DEADLINE / KP_ERR_CAPACITY of instance b.
+static int run_solve(kp_handle* h, int64_t deadline_ms, std::vector<int32_t>& statuses) {
+  const int n = (int)h->insts.size();
+  statuses.assign(n, KP_OK);
+  if (n == 0) return KP_OK;
   cudaSetDevice(h->device);
-  int rc = reset_dynamic(h);
-  if (rc != KP_OK) return rc;
+  if (n > h->devs_cap) {  // device copies of the pointer blocks and plans, grown on demand
+    cudaFree(h->d_devs);
+    cudaFree(h->d_plan);
+    h->d_devs = nullptr;
+    h->d_plan = nullptr;
+    h->devs_cap = 0;
+    CK(cudaMalloc(&h->d_devs, sizeof(KpDev) * n));
+    CK(cudaMalloc(&h->d_plan, sizeof(int2) * n));
+    h->devs_cap = n;
+  }
+  std::vector<KpDev> devs(n);
+  std::vector<int2> plan(n);
+  size_t smem = 0;
+  for (int b = 0; b < n; b++) {
+    Instance& in = *h->insts[b];
+    if (!in.resident) return h->err = "the last upload did not complete", KP_ERR_INVALID;
+    in.dev.deadline_ns = deadline_ms > 0 ? deadline_ms * 1000000ll : 0;
+    int rc = reset_dynamic(h, in);
+    if (rc != KP_OK) return rc;
+    devs[b] = in.dev;
+    plan[b] = make_int2(in.CS, in.CR);
+    smem = std::max(smem, in.smem);
+  }
+  CK(cudaMemcpyAsync(h->d_devs, devs.data(), sizeof(KpDev) * n, cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(h->d_plan, plan.data(), sizeof(int2) * n, cudaMemcpyHostToDevice, h->stream));
   CK(cudaEventRecord(h->ev0, h->stream));
   h->stats.kernel_launches = 0;
   h->stats.cohort_pods = 0;
-  rc = prep_solve(h);
-  if (rc != KP_OK) return rc;
-  const void* fn = in.lean ? (in.cohort ? (const void*)k_wsolve<true, true> : (const void*)k_wsolve<true, false>)
-                           : (in.cohort ? (const void*)k_wsolve<false, true> : (const void*)k_wsolve<false, false>);
-  if (in.host.has_vol_alts) fn = (const void*)k_wsolve<false, false, true>;
-  CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)in.smem));
-  CK(cudaEventRecord(h->ev2, h->stream));
+  for (auto& in : h->insts) {
+    int rc = prep_solve(h, *in);
+    if (rc != KP_OK) return rc;
+  }
+  const void* fn = solver_kernel(h->insts);
+  CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   {
-    void* args[] = {(void*)&d, (void*)&in.CS, (void*)&in.CR};
-    CK(cudaLaunchKernel(fn, dim3(1), dim3(64), args, in.smem, h->stream));
+    void* args[] = {(void*)&h->d_devs, (void*)&h->d_plan};
+    CK(cudaLaunchKernel(fn, dim3(n), dim3(64), args, smem, h->stream));
   }
   h->stats.kernel_launches++;
-  if (in.max_its > 0) {  // Results.TruncateInstanceTypes (scheduler.go:361-379)
-    k_truncate_claims<<<KP_TRUNC_BLOCKS, 128, 0, h->stream>>>(d, in.price_tabs, in.max_its, in.trunc_key, in.trunc_val, in.trunc_bits,
-                                                               in.d_dropped);
-    if (in.P > 0) k_mark_dropped<<<(int)((in.P + 255) / 256), 256, 0, h->stream>>>(d.pod_target, d.pod_error, in.d_dropped, in.P);
-    h->stats.kernel_launches += 2;
-  }
-  rc = reduce_counters(h, {&in});
+  for (auto& in : h->insts)
+    if (in->max_its > 0) {  // Results.TruncateInstanceTypes (scheduler.go:361-379)
+      k_truncate_claims<<<KP_TRUNC_BLOCKS, 128, 0, h->stream>>>(in->dev, in->price_tabs, in->max_its, in->trunc_key, in->trunc_val,
+                                                                 in->trunc_bits, in->d_dropped);
+      if (in->P > 0)
+        k_mark_dropped<<<(int)((in->P + 255) / 256), 256, 0, h->stream>>>(in->dev.pod_target, in->dev.pod_error, in->d_dropped, in->P);
+      h->stats.kernel_launches += 2;
+    }
+  int rc = reduce_counters(h);
   if (rc != KP_OK) return rc;
   CK(cudaEventRecord(h->ev1, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  CK(cudaStreamSynchronize(h->stream));  // devs / plan are host vectors: the copies above must have completed
   CK(cudaGetLastError());
   float ms = 0;
   cudaEventElapsedTime(&ms, h->ev0, h->ev1);
   h->stats.solve_ms = ms;
-  cudaEventElapsedTime(&in.wsolve_ms, h->ev2, h->ev1);
   if (h->d_gcnt) cudaEventElapsedTime(&h->allreduce_ms, h->ev3, h->ev1);
-  if (getenv("KP_DEBUG")) fprintf(stderr, "[kp] step %.3f ms, k_wsolve %.3f ms\n", ms, in.wsolve_ms);
+  if (getenv("KP_DEBUG")) fprintf(stderr, "[kp] %d instance(s): step %.3f ms\n", n, ms);
+  for (int b = 0; b < n; b++) CK(cudaMemcpy(&statuses[b], h->insts[b]->dev.status, 4, cudaMemcpyDeviceToHost));
   return KP_OK;
 }
 
-static int download(kp_handle* h, kp_result* out) {
-  KpDev& d = h->cur->dev;
+// The ABI's per-key requirement layout (kp_result.claim_req_*, kp_consol_result.repl_req_*): flags, gte and lte per key,
+// the mask of key k at word woff[k] of a row.  FinalizeScheduling drops the hostname requirement: it gets no mask words
+// and is never materialised as a slot here.
+struct ReqLayout {
+  int K, hostname_key;
+  std::vector<int> woff;  // [K + 1]
+  explicit ReqLayout(const Instance& in) : K(in.n_keys), hostname_key(in.hostname_key), woff(in.n_keys + 1, 0) {
+    for (int k = 0; k < K; k++) woff[k + 1] = woff[k] + (k == hostname_key ? 0 : (in.key_nvalues[k] + 63) / 64);
+  }
+  int words() const { return woff[K]; }
+  // the K device requirement slots of one claim -> row r of the ABI arrays (sg / sl null: the problem has no bounds)
+  void store(size_t r, const uint8_t* sf, const uint64_t* sm, const int64_t* sg, const int64_t* sl, uint8_t* flags,
+             int64_t* gte, int64_t* lte, uint64_t* mask) const {
+    for (int k = 0; k < K; k++) {
+      const uint8_t f = sf[k];
+      if (!(f & SF_PRESENT) || k == hostname_key) continue;
+      flags[r * K + k] = KP_SLOT_PRESENT | ((f & SF_COMPLEMENT) ? KP_REQ_COMPLEMENT : 0) | ((f & SF_HAS_GTE) ? KP_REQ_HAS_GTE : 0) |
+                         ((f & SF_HAS_LTE) ? KP_REQ_HAS_LTE : 0);
+      if ((f & SF_HAS_GTE) && sg) gte[r * K + k] = sg[k];
+      if ((f & SF_HAS_LTE) && sl) lte[r * K + k] = sl[k];
+      if (woff[k + 1] > woff[k]) mask[r * words() + woff[k]] = sm[k];
+    }
+  }
+};
+
+// Result of one instance after run_solve.  Adds to the handle's download stats.
+static int download(kp_handle* h, Instance& in, kp_result* out) {
+  KpDev& d = in.dev;
   auto t0 = std::chrono::steady_clock::now();
   memset(out, 0, sizeof(*out));
   int32_t nclaims = 0;
@@ -1104,8 +1196,8 @@ static int download(kp_handle* h, kp_result* out) {
   if (getenv("KP_DEBUG"))
     fprintf(stderr, "[kp] slow_sorts=%lld evals=%lld commits=%lld fast_commits=%lld cohort_pods=%lld\n", (long long)counters[4],
             (long long)counters[6], (long long)counters[3], (long long)counters[9], (long long)counters[5]);
-  int64_t P = h->cur->P;
-  int K = h->cur->n_keys, R = h->cur->n_resources, ITW = (h->cur->n_its + 63) / 64;
+  int64_t P = in.P;
+  int K = in.n_keys, R = in.n_resources, ITW = (in.n_its + 63) / 64;
   size_t C = (size_t)nclaims, c1 = C ? C : 1;
   out->n_pods = P;
   out->pod_target = (int32_t*)malloc(sizeof(int32_t) * (P ? P : 1));
@@ -1119,7 +1211,7 @@ static int download(kp_handle* h, kp_result* out) {
   out->claim_reservations = (uint64_t*)calloc(c1, 8);
   CK(cudaMemcpy(out->claim_reservations, d.c_rsv, C * 8, cudaMemcpyDeviceToHost));
   out->claim_dropped = (uint8_t*)calloc(c1, 1);
-  if (h->cur->d_dropped) CK(cudaMemcpy(out->claim_dropped, h->cur->d_dropped, C, cudaMemcpyDeviceToHost));
+  if (in.d_dropped) CK(cudaMemcpy(out->claim_dropped, in.d_dropped, C, cudaMemcpyDeviceToHost));
   out->claim_requests = (int64_t*)calloc(c1 * R, 8);
   out->it_words = ITW;
   out->claim_its = (uint64_t*)calloc(c1 * (ITW ? ITW : 1), 8);
@@ -1130,8 +1222,6 @@ static int download(kp_handle* h, kp_result* out) {
   std::vector<int32_t> order(c1);
   CK(cudaMemcpy(order.data(), d.order, C * 4, cudaMemcpyDeviceToHost));
   for (size_t pos = 0; pos < C; pos++) out->claim_rank[order[pos]] = (int32_t)pos;
-  // requirement slots -> the ABI's per-key layout (FinalizeScheduling drops the hostname requirement: it is never
-  // materialised as a slot here)
   std::vector<uint8_t> sf(c1 * K);
   std::vector<uint64_t> sm(c1 * K);
   std::vector<int64_t> sg(c1 * K), sl(c1 * K);
@@ -1139,9 +1229,8 @@ static int download(kp_handle* h, kp_result* out) {
   CK(cudaMemcpy(sm.data(), d.c_smask, C * K * 8, cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(sg.data(), d.c_sgte, C * K * 8, cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(sl.data(), d.c_slte, C * K * 8, cudaMemcpyDeviceToHost));
-  std::vector<int> woff(K + 1, 0);
-  for (int k = 0; k < K; k++) woff[k + 1] = woff[k] + (k == h->cur->hostname_key ? 0 : (h->cur->key_nvalues[k] + 63) / 64);
-  int MW = woff[K];
+  const ReqLayout L(in);
+  const int MW = L.words();
   out->n_keys = K;
   out->mask_words = MW;
   out->claim_req_flags = (uint8_t*)calloc(c1 * (K ? K : 1), 1);
@@ -1149,18 +1238,10 @@ static int download(kp_handle* h, kp_result* out) {
   out->claim_req_lte = (int64_t*)calloc(c1 * (K ? K : 1), 8);
   out->claim_req_mask = (uint64_t*)calloc(c1 * (MW ? MW : 1), 8);
   for (size_t c = 0; c < C; c++)
-    for (int k = 0; k < K; k++) {
-      uint8_t f = sf[c * K + k];
-      if (!(f & SF_PRESENT) || k == h->cur->hostname_key) continue;
-      uint8_t of = KP_SLOT_PRESENT | ((f & SF_COMPLEMENT) ? KP_REQ_COMPLEMENT : 0) |
-                   ((f & SF_HAS_GTE) ? KP_REQ_HAS_GTE : 0) | ((f & SF_HAS_LTE) ? KP_REQ_HAS_LTE : 0);
-      out->claim_req_flags[c * K + k] = of;
-      if (f & SF_HAS_GTE) out->claim_req_gte[c * K + k] = sg[c * K + k];
-      if (f & SF_HAS_LTE) out->claim_req_lte[c * K + k] = sl[c * K + k];
-      if (woff[k + 1] > woff[k]) out->claim_req_mask[c * MW + woff[k]] = sm[c * K + k];
-    }
+    L.store(c, sf.data() + c * K, sm.data() + c * K, sg.data() + c * K, sl.data() + c * K, out->claim_req_flags,
+            out->claim_req_gte, out->claim_req_lte, out->claim_req_mask);
   // topology counters, non-hostname groups (regular then inverse == creation order of the reference's two maps)
-  HostTables& t = h->cur->host;
+  HostTables& t = in.host;
   std::vector<int32_t> cnt((size_t)std::max(t.G, 1) * 64);
   CK(cudaMemcpy(cnt.data(), d.dom_cnt, cnt.size() * 4, cudaMemcpyDeviceToHost));
   // order of the reference's maps: groups of NewTopology in creation order, then the groups relaxed pods created, in
@@ -1182,7 +1263,7 @@ static int download(kp_handle* h, kp_result* out) {
   for (int g : gorder) {
     int key = t.groups[g].key;
     if (key != t.hostname_key) {
-      int nv = h->cur->key_nvalues[key];
+      int nv = in.key_nvalues[key];
       for (int v = 0; v < nv; v++) flat.push_back(cnt[(size_t)g * 64 + v]);
     }
     off.push_back((int32_t)flat.size());
@@ -1198,39 +1279,70 @@ static int download(kp_handle* h, kp_result* out) {
   out->n_template_evals = counters[2];
   out->n_commits = counters[3];
   out->solve_ms = h->stats.solve_ms;
-  h->stats.bytes_d2h = P * 5 + C * (8 + (size_t)R * 8 + (size_t)ITW * 8 + (size_t)K * 25) + cnt.size() * 4;
+  h->stats.bytes_d2h += P * 5 + C * (8 + (size_t)R * 8 + (size_t)ITW * 8 + (size_t)K * 25) + cnt.size() * 4;
   auto t1 = std::chrono::steady_clock::now();
-  h->stats.download_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
+  h->stats.download_ms += std::chrono::duration<double, std::milli>(t1 - t0).count();
   return KP_OK;
 }
 
-int kp_solve_resident(kp_handle* h, int64_t deadline_ms, kp_result* out) {
-  h->cur->dev.deadline_ns = deadline_ms > 0 ? deadline_ms * 1000000ll : 0;
-  if (!h->cur->resident) return h->err = "kp_upload has not been called", KP_ERR_INVALID;
-  int rc = run_solve(h);
-  if (rc != KP_OK) return rc;
-  int32_t status = 0;
-  CK(cudaMemcpy(&status, h->cur->dev.status, 4, cudaMemcpyDeviceToHost));
-  if (status == KP_DEADLINE) {  // partial results are valid (scheduler.go:411-414)
-    rc = download(h, out);
-    return rc == KP_OK ? KP_DEADLINE : rc;
+// outs[b] <- instance b after run_solve; KP_DEADLINE when some instance ran out of time (partial results are valid,
+// scheduler.go:411-414)
+static int download_all(kp_handle* h, const std::vector<int32_t>& statuses, kp_result* outs) {
+  h->stats.download_ms = 0;
+  h->stats.bytes_d2h = 0;
+  int worst = KP_OK;
+  for (size_t b = 0; b < h->insts.size(); b++) {
+    int rc = download(h, *h->insts[b], &outs[b]);
+    if (rc != KP_OK) {
+      for (size_t i = 0; i < b; i++) kp_result_free(&outs[i]);
+      return rc;
+    }
+    if (statuses[b] == KP_DEADLINE) worst = KP_DEADLINE;
   }
-  if (status != KP_OK) return h->err = "claim capacity exceeded", status;
-  return download(h, out);
+  return worst;
+}
+
+static int solve_uploaded(kp_handle* h, int64_t deadline_ms, kp_result* outs) {
+  std::vector<int32_t> st;
+  int rc = run_solve(h, deadline_ms, st);
+  if (rc != KP_OK) return rc;
+  for (int32_t s : st)
+    if (s != KP_OK && s != KP_DEADLINE) return h->err = "claim capacity exceeded", s;
+  return download_all(h, st, outs);
+}
+
+// kp_solve / kp_solve_batch: upload, solve, and while some instance needs more NodeClaims than provisioned, grow its
+// claim capacity and redo
+static int solve_growing(kp_handle* h, const kp_problem* const* problems, int n, kp_handle::Uploader by, int64_t deadline_ms,
+                         kp_result* outs) {
+  std::vector<int64_t> cmax(n);
+  for (int b = 0; b < n; b++) cmax[b] = cmax_guess(problems[b]);
+  for (;;) {
+    int rc = upload(h, problems, n, cmax.data(), by);
+    if (rc != KP_OK) return rc;
+    std::vector<int32_t> st;
+    rc = run_solve(h, deadline_ms, st);
+    if (rc != KP_OK) return rc;
+    bool grow = false;
+    for (int b = 0; b < n; b++) {
+      if (st[b] == KP_ERR_CAPACITY && cmax[b] < problems[b]->n_pods) {
+        cmax[b] = std::min<int64_t>(problems[b]->n_pods, cmax[b] * 4);
+        grow = true;
+      } else if (st[b] != KP_OK && st[b] != KP_DEADLINE) {
+        return h->err = "claim capacity exceeded", st[b];
+      }
+    }
+    if (!grow) return download_all(h, st, outs);
+  }
+}
+
+int kp_solve_resident(kp_handle* h, int64_t deadline_ms, kp_result* out) {
+  if (h->uploaded != kp_handle::SINGLE) return h->err = "kp_upload has not been called", KP_ERR_INVALID;
+  return solve_uploaded(h, deadline_ms, out);
 }
 
 int kp_solve(kp_handle* h, const kp_problem* p, int64_t deadline_ms, kp_result* out) {
-  int64_t cmax = std::min<int64_t>(p->n_pods, std::max<int64_t>(4096, p->n_pods / 8));
-  for (;;) {
-    int rc = do_upload(h, p, (int)std::max<int64_t>(cmax, 1));
-    if (rc != KP_OK) return rc;
-    rc = kp_solve_resident(h, deadline_ms, out);
-    if (rc == KP_ERR_CAPACITY && cmax < p->n_pods) {  // more NodeClaims than provisioned: grow and redo
-      cmax = std::min<int64_t>(p->n_pods, cmax * 4);
-      continue;
-    }
-    return rc;
-  }
+  return solve_growing(h, &p, 1, kp_handle::SINGLE, deadline_ms, out);
 }
 
 // ---- multi-GPU: the global topology-domain counter table of a NodePool-sharded job --------------------------------
@@ -1263,8 +1375,9 @@ int kp_comm_init(kp_handle* h, const uint8_t* id128, int32_t rank, int32_t world
 // the inverse groups), one slot per value of the group's key -- the layout of kp_result.domain_counts when no group is
 // born mid-solve.  instance < 0: the kp_upload instance, else index into the kp_upload_batch list.
 static Instance* pick_instance(kp_handle* h, int32_t instance) {
-  if (instance < 0) return h->main.resident ? &h->main : nullptr;
-  return instance < (int)h->batch.size() ? h->batch[instance] : nullptr;
+  const size_t i = instance < 0 ? 0 : (size_t)instance;
+  if (h->uploaded != (instance < 0 ? kp_handle::SINGLE : kp_handle::BATCH) || i >= h->insts.size()) return nullptr;
+  return h->insts[i]->resident ? h->insts[i].get() : nullptr;
 }
 int64_t kp_comm_counter_slots(kp_handle* h, int32_t instance) {
   Instance* in = pick_instance(h, instance);
@@ -1280,19 +1393,13 @@ int64_t kp_comm_counter_slots(kp_handle* h, int32_t instance) {
 // kp_solve_batch_resident ends with scatter + all-reduce (when kp_comm_init was called) inside its solve_ms.
 int kp_comm_set_counter_layout(kp_handle* h, int64_t total_slots, const int64_t* slot_offset, int32_t n_instances) {
   cudaSetDevice(h->device);
-  std::vector<Instance*> insts;
-  if (n_instances <= 0) {
-    if (!h->main.resident) return h->err = "kp_comm_set_counter_layout: nothing uploaded", KP_ERR_INVALID;
-    insts.push_back(&h->main);
-  } else {
-    if (n_instances != (int)h->batch.size()) return h->err = "kp_comm_set_counter_layout: batch size mismatch", KP_ERR_INVALID;
-    insts = h->batch;
-  }
+  if (n_instances <= 0 ? !pick_instance(h, -1) : h->uploaded != kp_handle::BATCH || n_instances != (int)h->insts.size())
+    return h->err = "kp_comm_set_counter_layout: the instances do not match the upload", KP_ERR_INVALID;
   if (total_slots < 0) return h->err = "kp_comm_set_counter_layout: negative size", KP_ERR_INVALID;
   CK(h->arena.alloc(&h->d_gcnt, (size_t)std::max<int64_t>(total_slots, 1)));
   h->gcnt_slots = total_slots;
-  for (size_t i = 0; i < insts.size(); i++) {
-    Instance* in = insts[i];
+  for (size_t i = 0; i < h->insts.size(); i++) {
+    Instance* in = h->insts[i].get();
     std::vector<int32_t> src;
     for (int g = 0; g < in->host.G; g++) {
       const int key = in->host.groups[g].key;
@@ -1325,178 +1432,21 @@ void kp_comm_destroy(kp_handle* h) {
 }
 
 // ---- kp_solve_batch: n independent Scheduler instances, one launch (one CTA per instance) ------------------------
-static void batch_clear(kp_handle* h) {
-  for (Instance* b : h->batch) delete b;
-  h->batch.clear();
-  h->cur = &h->main;
-}
-
-static int upload_batch(kp_handle* h, const kp_problem* const* problems, int n, const std::vector<int64_t>& cmax) {
-  batch_clear(h);
-  h->main.resident = false;
-  double prep = 0, upl = 0;
-  int64_t h2d = 0;
-  for (int b = 0; b < n; b++) {
-    h->batch.push_back(new Instance());
-    h->cur = h->batch.back();
-    int rc = do_upload(h, problems[b], (int)std::max<int64_t>(cmax[b], 1), b == 0);
-    prep += h->stats.prep_ms;
-    upl += h->stats.upload_ms;
-    h2d += h->stats.bytes_h2d;
-    if (rc != KP_OK) {
-      h->cur = &h->main;
-      return rc;
-    }
-  }
-  h->cur = &h->main;
-  h->stats.prep_ms = prep;
-  h->stats.upload_ms = upl;
-  h->stats.bytes_h2d = h2d;
-  CK(h->arena.alloc(&h->d_batch_devs, (size_t)std::max(n, 1)));
-  CK(h->arena.alloc(&h->d_batch_plan, (size_t)std::max(n, 1)));
-  return KP_OK;
-}
-
-static int64_t cmax_guess(const kp_problem* p) {
-  return std::min<int64_t>(p->n_pods, std::max<int64_t>(4096, p->n_pods / 8));
-}
-
 int kp_upload_batch(kp_handle* h, const kp_problem* const* problems, int32_t n) {
   if (n < 0 || (n > 0 && !problems)) return h->err = "kp_upload_batch: bad arguments", KP_ERR_INVALID;
   std::vector<int64_t> cmax(n);
   for (int b = 0; b < n; b++) cmax[b] = cmax_guess(problems[b]);
-  return upload_batch(h, problems, n, cmax);
-}
-
-// statuses[b]: KP_OK / KP_DEADLINE / KP_ERR_CAPACITY of instance b
-static int run_batch(kp_handle* h, int64_t deadline_ms, std::vector<int32_t>& statuses) {
-  const int n = (int)h->batch.size();
-  statuses.assign(n, KP_OK);
-  if (n == 0) return KP_OK;
-  cudaSetDevice(h->device);
-  for (Instance* b : h->batch) {
-    if (!b->resident) return h->err = "kp_upload_batch has not been called", KP_ERR_INVALID;
-    b->dev.deadline_ns = deadline_ms > 0 ? deadline_ms * 1000000ll : 0;
-    h->cur = b;
-    int rc = reset_dynamic(h);
-    if (rc != KP_OK) return h->cur = &h->main, rc;
-  }
-  CK(cudaEventRecord(h->ev0, h->stream));
-  h->stats.kernel_launches = 0;
-  h->stats.cohort_pods = 0;
-  std::vector<KpDev> devs(n);
-  std::vector<int2> plan(n);
-  size_t smem = 0;
-  for (int b = 0; b < n; b++) {
-    h->cur = h->batch[b];
-    int rc = prep_solve(h);
-    if (rc != KP_OK) return h->cur = &h->main, rc;
-    devs[b] = h->cur->dev;
-    plan[b] = make_int2(h->cur->CS, h->cur->CR);
-    smem = std::max(smem, h->cur->smem);
-  }
-  h->cur = &h->main;
-  CK(cudaMemcpyAsync(h->d_batch_devs, devs.data(), sizeof(KpDev) * n, cudaMemcpyHostToDevice, h->stream));
-  CK(cudaMemcpyAsync(h->d_batch_plan, plan.data(), sizeof(int2) * n, cudaMemcpyHostToDevice, h->stream));
-  bool all_lean = true, any_cohort = false;
-  for (Instance* b : h->batch) {
-    all_lean = all_lean && b->lean;
-    any_cohort = any_cohort || b->cohort;
-  }
-  bool any_vol = false;
-  for (Instance* b : h->batch) any_vol = any_vol || b->host.has_vol_alts;
-  if (any_vol) any_cohort = false;
-  const void* fn = all_lean ? (any_cohort ? (const void*)k_wsolve_batch<true, true> : (const void*)k_wsolve_batch<true, false>)
-                            : (any_cohort ? (const void*)k_wsolve_batch<false, true> : (const void*)k_wsolve_batch<false, false>);
-  if (any_vol) fn = (const void*)k_wsolve_batch<false, false, true>;
-  CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  CK(cudaEventRecord(h->ev2, h->stream));
-  {
-    void* args[] = {(void*)&h->d_batch_devs, (void*)&h->d_batch_plan};
-    CK(cudaLaunchKernel(fn, dim3(n), dim3(64), args, smem, h->stream));
-  }
-  h->stats.kernel_launches++;
-  for (Instance* b : h->batch)
-    if (b->max_its > 0) {
-      k_truncate_claims<<<KP_TRUNC_BLOCKS, 128, 0, h->stream>>>(b->dev, b->price_tabs, b->max_its, b->trunc_key, b->trunc_val,
-                                                                 b->trunc_bits, b->d_dropped);
-      if (b->P > 0) k_mark_dropped<<<(int)((b->P + 255) / 256), 256, 0, h->stream>>>(b->dev.pod_target, b->dev.pod_error, b->d_dropped, b->P);
-      h->stats.kernel_launches += 2;
-    }
-  {
-    int rc = reduce_counters(h, h->batch);
-    if (rc != KP_OK) return rc;
-  }
-  CK(cudaEventRecord(h->ev1, h->stream));
-  CK(cudaStreamSynchronize(h->stream));  // devs / plan are host vectors: the copies above must have completed
-  CK(cudaGetLastError());
-  float ms = 0, wms = 0;
-  cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-  cudaEventElapsedTime(&wms, h->ev2, h->ev1);
-  h->stats.solve_ms = ms;
-  if (h->d_gcnt) cudaEventElapsedTime(&h->allreduce_ms, h->ev3, h->ev1);
-  if (getenv("KP_DEBUG")) fprintf(stderr, "[kp] batch of %d: step %.3f ms, k_wsolve_batch %.3f ms\n", n, ms, wms);
-  for (int b = 0; b < n; b++) {
-    h->batch[b]->wsolve_ms = wms;
-    CK(cudaMemcpy(&statuses[b], h->batch[b]->dev.status, 4, cudaMemcpyDeviceToHost));
-  }
-  return KP_OK;
-}
-
-static int download_batch(kp_handle* h, const std::vector<int32_t>& statuses, kp_result* outs) {
-  int worst = KP_OK;
-  double dl = 0;
-  int64_t d2h = 0;
-  const double solve_ms = h->stats.solve_ms;
-  for (size_t b = 0; b < h->batch.size(); b++) {
-    h->cur = h->batch[b];
-    int rc = download(h, &outs[b]);
-    h->cur = &h->main;
-    if (rc != KP_OK) {
-      for (size_t i = 0; i < b; i++) kp_result_free(&outs[i]);
-      return rc;
-    }
-    outs[b].solve_ms = solve_ms;
-    dl += h->stats.download_ms;
-    d2h += h->stats.bytes_d2h;
-    if (statuses[b] == KP_DEADLINE) worst = KP_DEADLINE;
-  }
-  h->stats.download_ms = dl;
-  h->stats.bytes_d2h = d2h;
-  return worst;
+  return upload(h, problems, n, cmax.data(), kp_handle::BATCH);
 }
 
 int kp_solve_batch_resident(kp_handle* h, int64_t deadline_ms, kp_result* outs) {
-  std::vector<int32_t> st;
-  int rc = run_batch(h, deadline_ms, st);
-  if (rc != KP_OK) return rc;
-  for (int32_t s : st)
-    if (s != KP_OK && s != KP_DEADLINE) return h->err = "claim capacity exceeded in a batch instance", s;
-  return download_batch(h, st, outs);
+  if (h->uploaded != kp_handle::BATCH) return KP_OK;  // nothing from kp_upload_batch: an empty batch
+  return solve_uploaded(h, deadline_ms, outs);
 }
 
 int kp_solve_batch(kp_handle* h, const kp_problem* const* problems, int32_t n, int64_t deadline_ms, kp_result* outs) {
   if (n < 0 || (n > 0 && (!problems || !outs))) return h->err = "kp_solve_batch: bad arguments", KP_ERR_INVALID;
-  std::vector<int64_t> cmax(n);
-  for (int b = 0; b < n; b++) cmax[b] = cmax_guess(problems[b]);
-  for (;;) {
-    int rc = upload_batch(h, problems, n, cmax);
-    if (rc != KP_OK) return rc;
-    std::vector<int32_t> st;
-    rc = run_batch(h, deadline_ms, st);
-    if (rc != KP_OK) return rc;
-    bool grow = false;
-    for (int b = 0; b < n; b++) {
-      if (st[b] == KP_ERR_CAPACITY && cmax[b] < problems[b]->n_pods) {  // more NodeClaims than provisioned: grow, redo
-        cmax[b] = std::min<int64_t>(problems[b]->n_pods, cmax[b] * 4);
-        grow = true;
-      } else if (st[b] != KP_OK && st[b] != KP_DEADLINE) {
-        return h->err = "batch instance failed", st[b];
-      }
-    }
-    if (grow) continue;
-    return download_batch(h, st, outs);
-  }
+  return solve_growing(h, problems, n, kp_handle::BATCH, deadline_ms, outs);
 }
 
 void kp_result_free(kp_result* r) {
@@ -1519,9 +1469,10 @@ void kp_result_free(kp_result* r) {
 }
 
 int kp_feasibility(kp_handle* h, const kp_problem* p, uint64_t* out_bits, int32_t* out_it_words) {
-  int rc = do_upload(h, p, 1);
+  const int64_t one = 1;
+  int rc = upload(h, &p, 1, &one, kp_handle::SINGLE);
   if (rc != KP_OK) return rc;
-  KpDev& d = h->cur->dev;
+  KpDev& d = h->insts[0]->dev;
   *out_it_words = d.ITW;
   size_t n = (size_t)d.X * d.N * d.ITW;
   uint64_t* dout;
@@ -1573,6 +1524,53 @@ __global__ void k_scatter_rank(const int32_t* perm, int64_t n, int32_t* rank) {
   if (i < n) rank[perm[i]] = (int32_t)i;
 }
 
+// Rows [0, n) of the KpConsol outputs -> subsets at[0, n) of `out` (at null: row b is subset b, and the fixed-size
+// fields are copied in place); with the price-order export, the orders go to order_rows
+static int read_consol(kp_handle* h, const KpConsol& q, int n, const int32_t* at, const ReqLayout& L, int R, int ITW,
+                       std::vector<std::vector<int32_t>>& order_rows, kp_consol_result* out) {
+  const size_t K = (size_t)L.K, n1 = (size_t)std::max(n, 1), cap = (size_t)q.order_cap;
+  auto sub = [&](size_t b) { return at ? (size_t)at[b] : b; };
+  auto rows = [&](auto* dst, const auto* src, size_t width) {  // `width` elements per row
+    const size_t row = width * sizeof(*dst);
+    if (!at) return cudaMemcpy(dst, src, n * row, cudaMemcpyDeviceToHost);
+    std::vector<std::remove_pointer_t<decltype(dst)>> tmp(n1 * width);
+    const cudaError_t e = cudaMemcpy(tmp.data(), src, n * row, cudaMemcpyDeviceToHost);
+    for (size_t b = 0; b < (size_t)n; b++) memcpy(dst + sub(b) * width, tmp.data() + b * width, row);
+    return e;
+  };
+  CK(rows(out->decision, q.decision, 1));
+  CK(rows(out->replacement_its, q.replacement_its, ITW));
+  CK(rows(out->n_new_claims, q.n_new_claims, 1));
+  CK(rows(out->n_unscheduled, q.n_unscheduled, 1));
+  CK(rows(out->repl_template, q.repl_tmpl, 1));
+  CK(rows(out->repl_requests, q.repl_req, R));
+  std::vector<uint8_t> sfl(n1 * K);
+  std::vector<uint64_t> smk(n1 * K);
+  std::vector<int32_t> on(n1), ord(q.repl_order ? n1 * cap : 0);
+  std::vector<int64_t> sg(q.repl_sgte ? n1 * K : 0), sl(sg.size());
+  CK(cudaMemcpy(sfl.data(), q.repl_sflags, (size_t)n * K, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(smk.data(), q.repl_smask, (size_t)n * K * 8, cudaMemcpyDeviceToHost));
+  if (q.repl_sgte) {
+    CK(cudaMemcpy(sg.data(), q.repl_sgte, (size_t)n * K * 8, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(sl.data(), q.repl_slte, (size_t)n * K * 8, cudaMemcpyDeviceToHost));
+  }
+  if (q.repl_order) {
+    CK(cudaMemcpy(ord.data(), q.repl_order, (size_t)n * cap * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(on.data(), q.repl_order_n, (size_t)n * 4, cudaMemcpyDeviceToHost));
+  }
+  for (size_t b = 0; b < (size_t)n; b++) {
+    const size_t s = sub(b);
+    if (out->decision[s] != KP_DECISION_REPLACE)
+      out->repl_template[s] = -1;
+    else
+      L.store(s, sfl.data() + b * K, smk.data() + b * K, q.repl_sgte ? sg.data() + b * K : nullptr,
+              q.repl_sgte ? sl.data() + b * K : nullptr, out->repl_req_flags, out->repl_req_gte, out->repl_req_lte,
+              out->repl_req_mask);
+    if (q.repl_order) order_rows[s].assign(ord.begin() + b * cap, ord.begin() + b * cap + on[b]);
+  }
+  return KP_OK;
+}
+
 // kp_consolidate: every subset is one SimulateScheduling + computeConsolidation (helpers.go:51-142,
 // consolidation.go:136-229); they are independent, so each runs as its own solver instance on its own warp.
 static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_consol_input* in, int64_t deadline_ms,
@@ -1587,10 +1585,12 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   for (int i = 0; i < n_extra; i++)
     if (in->extra_pod_kind[i] != KP_EXTRA_PENDING && in->extra_pod_kind[i] != KP_EXTRA_DELETING_NODE)
       return h->err = "kp_consolidate: unknown extra pod kind", KP_ERR_INVALID;
-  int rc = do_upload(h, p, 1);  // the cluster's pod table doubles as the "pods" of the problem (rows by node)
+  const int64_t one = 1;
+  int rc = upload(h, &p, 1, &one, kp_handle::SINGLE);  // the cluster's pod table doubles as the "pods" of the problem (rows by node)
   if (rc != KP_OK) return rc;
-  HostTables& t = h->cur->host;
-  KpDev& d = h->cur->dev;
+  Instance& cl = *h->insts[0];
+  HostTables& t = cl.host;
+  KpDev& d = cl.dev;
   if (t.has_vol_alts) {
     h->err = "consolidation with pods that have several volume-topology alternatives is not supported yet";
     return KP_ERR_UNSUPPORTED;
@@ -1603,12 +1603,9 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   }
   const int K = t.K, R = t.R, ITW = t.ITW, E = t.E, N = t.N, T = t.T;
   const bool general = t.G > 0;  // the evicted pods carry topology constraints: one full solve per candidate set
-  const std::vector<int> key_nvalues = h->cur->key_nvalues;
-  const int hostname_key = h->cur->hostname_key;
+  const ReqLayout L(cl);
   // ---- result arrays (owned by `out` from here on: kp_consolidate frees them on any error return)
-  std::vector<int> woff(p->n_keys + 1, 0);
-  for (int k = 0; k < p->n_keys; k++) woff[k + 1] = woff[k] + (k == hostname_key ? 0 : (key_nvalues[k] + 63) / 64);
-  const int MW = woff[p->n_keys];
+  const int MW = L.words();
   {
     const size_t s1 = S ? S : 1;
     out->n_subsets = S;
@@ -1631,18 +1628,6 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   }
   const int order_cap = std::min(std::max(T, 1), 600);
   std::vector<std::vector<int32_t>> order_rows(in->export_price_order ? S : 0);
-  // device slots of a replacement claim -> the ABI's per-key layout (as download() does for kp_result.claim_req_*)
-  auto store_repl = [&](int s_out, const uint8_t* sf, const uint64_t* sm, const int64_t* sg, const int64_t* sl) {
-    for (int k = 0; k < K; k++) {
-      const uint8_t f = sf[k];
-      if (!(f & SF_PRESENT) || k == hostname_key) continue;
-      out->repl_req_flags[(size_t)s_out * K + k] = KP_SLOT_PRESENT | ((f & SF_COMPLEMENT) ? KP_REQ_COMPLEMENT : 0) |
-                                                   ((f & SF_HAS_GTE) ? KP_REQ_HAS_GTE : 0) | ((f & SF_HAS_LTE) ? KP_REQ_HAS_LTE : 0);
-      if ((f & SF_HAS_GTE) && sg) out->repl_req_gte[(size_t)s_out * K + k] = sg[k];
-      if ((f & SF_HAS_LTE) && sl) out->repl_req_lte[(size_t)s_out * K + k] = sl[k];
-      if (woff[k + 1] > woff[k]) out->repl_req_mask[(size_t)s_out * MW + woff[k]] = sm[k];
-    }
-  };
   auto finish_order = [&]() {
     if (!in->export_price_order) return;
     out->repl_order_off = (int32_t*)calloc((size_t)S + 1, 4);
@@ -1719,25 +1704,7 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
     wl_set.push_back(0);
     wl_price.push_back(0);
   }
-  // OrderByPrice lists: available offerings per instance type, cheapest first
-  std::vector<int32_t> ml_off((size_t)T + 1, 0), ml_set;
-  std::vector<double> ml_price;
-  for (int ti = 0; ti < T; ti++) {
-    std::vector<std::pair<double, int>> ent;
-    for (int o = p->it_off_off[ti]; o < p->it_off_off[ti + 1]; o++)
-      if (p->off_available[o]) ent.push_back({p->off_price[o], t.off_set[o]});
-    std::stable_sort(ent.begin(), ent.end(),
-                     [](const std::pair<double, int>& a, const std::pair<double, int>& b) { return a.first < b.first; });
-    for (auto& e : ent) {
-      ml_price.push_back(e.first);
-      ml_set.push_back(e.second);
-    }
-    ml_off[(size_t)ti + 1] = (int32_t)ml_set.size();
-  }
-  if (ml_set.empty()) {
-    ml_set.push_back(0);
-    ml_price.push_back(0);
-  }
+  const PriceLists ml = order_by_price(p, t);
   // price tables and decision constants of the device side (both paths)
   auto upload_prices = [&](KpConsol& q) -> int {
     q.ct_key = in->capacity_type_key;
@@ -1756,9 +1723,9 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
     CK(up_raw(h, &nit, in->node_it, (size_t)E));
     q.node_it = nit;
     q.filter_same_type = in->filter_same_instance_type;
-    CK(up(h, &q.ml_off, ml_off));
-    CK(up(h, &q.ml_set, ml_set));
-    CK(up(h, &q.ml_price, ml_price));
+    CK(up(h, &q.ml_off, ml.off));
+    CK(up(h, &q.ml_set, ml.set));
+    CK(up(h, &q.ml_price, ml.price));
     CK(up(h, &q.wl_off, wl_off));
     CK(up(h, &q.wl_set, wl_set));
     CK(up(h, &q.wl_price, wl_price));
@@ -1773,7 +1740,12 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   if (general) {
     // ---- general path: a candidate set is SimulateScheduling over its own stateNodes / bound pods / pending pods
     // (helpers.go:51-142) -> a derived kp_problem (fresh NewTopology).  All sets of a chunk are uploaded side by side and
-    // solved by ONE k_wsolve_batch launch (one CTA per set), then k_decide_batch applies computeConsolidation.
+    // solved by ONE k_wsolve_batch launch (one CTA per set), then k_decide_batch applies computeConsolidation.  Each
+    // chunk's upload replaces the handle's instances and reuses the arena: from then on only the cluster's host tables
+    // are read.
+    const std::unique_ptr<Instance> cluster = std::move(h->insts[0]);
+    h->insts.clear();
+    h->uploaded = kp_handle::NONE;
     double total_ms = 0;
     bool timed_out = false;
     const int CHUNK = 2 * h->n_sm;  // two waves of CTAs; bounds the HBM the side-by-side tables take
@@ -1784,10 +1756,9 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
         timed_out = true;
         break;
       }
-      batch_clear(h);
+      begin_upload(h, kp_handle::NONE);  // the sets of a chunk are no upload kp_solve_resident / kp_solve_batch_resident serve
       std::vector<int> set_of;  // instance -> subset
       std::vector<int32_t> soff{0}, snodes_all;
-      bool first = true;
       for (int s = c0; s < c1; s++) {
         const int so = in->subset_off[s], sn = in->subset_off[s + 1] - so;
         std::fill(is_cand.begin(), is_cand.end(), 0);
@@ -1830,33 +1801,24 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
         sp.n_running = (int64_t)run_class.size();
         sp.run_class = run_class.data();
         sp.run_node = run_node.data();
-        h->batch.push_back(new Instance());
-        h->cur = h->batch.back();
-        rc = do_upload(h, &sp, (int)std::max<int64_t>(sp.n_pods, 1), first);
-        if (rc == KP_OK && n_extra > 0) {
-          uint8_t* dk;
-          cudaError_t e = up_raw(h, &dk, kinds.data(), kinds.size());
-          if (e != cudaSuccess) rc = (h->err = cudaGetErrorString(e), KP_ERR_CUDA);
-          h->cur->dev.pod_kind = dk;
-          cudaStreamSynchronize(h->stream);  // `kinds` dies with this iteration
-        }
-        h->cur = &h->main;
+        rc = add_instance(h, &sp, sp.n_pods);
         if (rc != KP_OK) return rc;
-        first = false;
+        if (n_extra > 0) {
+          uint8_t* dk;
+          CK(up_raw(h, &dk, kinds.data(), kinds.size()));
+          h->insts.back()->dev.pod_kind = dk;
+          CK(cudaStreamSynchronize(h->stream));  // `kinds` dies with this iteration
+        }
         set_of.push_back(s);
         for (int i = 0; i < sn; i++) snodes_all.push_back(in->subset_nodes[so + i]);
         soff.push_back((int32_t)snodes_all.size());
       }
       const int nb = (int)set_of.size();
       if (nb == 0) continue;
-      h->cur = h->batch[0];  // upload_prices / arena helpers account their bytes on the current instance's handle stats
       KpConsol q;
       memset(&q, 0, sizeof(q));
       rc = upload_prices(q);
-      h->cur = &h->main;
       if (rc != KP_OK) return rc;
-      CK(h->arena.alloc(&h->d_batch_devs, (size_t)nb));
-      CK(h->arena.alloc(&h->d_batch_plan, (size_t)nb));
       int32_t *d_soff, *d_snodes;
       CK(up_raw(h, &d_soff, soff.data(), soff.size()));
       CK(up_raw(h, &d_snodes, snodes_all.data(), std::max<size_t>(snodes_all.size(), 1)));
@@ -1881,7 +1843,7 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
         CK(zeros(h, &q.repl_order_n, nb1));
       }
       std::vector<int32_t> st;
-      rc = run_batch(h, ms_left() < 0 ? 0 : std::max<int64_t>(ms_left(), 1), st);
+      rc = run_solve(h, ms_left() < 0 ? 0 : std::max<int64_t>(ms_left(), 1), st);
       if (rc != KP_OK) return rc;
       total_ms += h->stats.solve_ms;
       bool chunk_timed_out = false;
@@ -1895,47 +1857,13 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
         timed_out = true;
         break;
       }
-      k_decide_batch<<<nb, 32, 0, h->stream>>>(h->d_batch_devs, q, d_soff, d_snodes);
+      k_decide_batch<<<nb, 32, 0, h->stream>>>(h->d_devs, q, d_soff, d_snodes);
       CK(cudaStreamSynchronize(h->stream));
       CK(cudaGetLastError());
-      std::vector<uint8_t> dec(nb), sfl(nb1 * K);
-      std::vector<uint64_t> rep(nb1 * std::max(ITW, 1)), smk(nb1 * K);
-      std::vector<int32_t> nn(nb), nu(nb), rt(nb), on(nb), ord;
-      std::vector<int64_t> rq(nb1 * R), sg, sl;
-      CK(cudaMemcpy(dec.data(), q.decision, nb1, cudaMemcpyDeviceToHost));
-      CK(cudaMemcpy(rep.data(), q.replacement_its, nb1 * ITW * 8, cudaMemcpyDeviceToHost));
-      CK(cudaMemcpy(nn.data(), q.n_new_claims, nb1 * 4, cudaMemcpyDeviceToHost));
-      CK(cudaMemcpy(nu.data(), q.n_unscheduled, nb1 * 4, cudaMemcpyDeviceToHost));
-      CK(cudaMemcpy(rt.data(), q.repl_tmpl, nb1 * 4, cudaMemcpyDeviceToHost));
-      CK(cudaMemcpy(rq.data(), q.repl_req, nb1 * R * 8, cudaMemcpyDeviceToHost));
-      CK(cudaMemcpy(sfl.data(), q.repl_sflags, nb1 * K, cudaMemcpyDeviceToHost));
-      CK(cudaMemcpy(smk.data(), q.repl_smask, nb1 * K * 8, cudaMemcpyDeviceToHost));
-      if (t.has_bounds) {
-        sg.resize(nb1 * K);
-        sl.resize(nb1 * K);
-        CK(cudaMemcpy(sg.data(), q.repl_sgte, nb1 * K * 8, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(sl.data(), q.repl_slte, nb1 * K * 8, cudaMemcpyDeviceToHost));
-      }
-      if (in->export_price_order) {
-        ord.resize(nb1 * order_cap);
-        CK(cudaMemcpy(ord.data(), q.repl_order, nb1 * order_cap * 4, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(on.data(), q.repl_order_n, nb1 * 4, cudaMemcpyDeviceToHost));
-      }
-      for (int b_ = 0; b_ < nb; b_++) {
-        const int s = set_of[b_];
-        out->decision[s] = dec[b_];
-        memcpy(out->replacement_its + (size_t)s * ITW, rep.data() + (size_t)b_ * ITW, (size_t)ITW * 8);
-        out->n_new_claims[s] = nn[b_];
-        out->n_unscheduled[s] = nu[b_];
-        out->repl_template[s] = rt[b_];
-        memcpy(out->repl_requests + (size_t)s * R, rq.data() + (size_t)b_ * R, (size_t)R * 8);
-        if (dec[b_] == KP_DECISION_REPLACE)
-          store_repl(s, sfl.data() + (size_t)b_ * K, smk.data() + (size_t)b_ * K, t.has_bounds ? sg.data() + (size_t)b_ * K : nullptr,
-                     t.has_bounds ? sl.data() + (size_t)b_ * K : nullptr);
-        if (in->export_price_order) order_rows[s].assign(ord.begin() + (size_t)b_ * order_cap, ord.begin() + (size_t)b_ * order_cap + on[b_]);
-      }
+      rc = read_consol(h, q, nb, set_of.data(), L, R, ITW, order_rows, out);
+      if (rc != KP_OK) return rc;
     }
-    batch_clear(h);
+    h->insts.clear();
     finish_order();
     out->solve_ms = total_ms;
     h->stats.solve_ms = total_ms;
@@ -1965,7 +1893,7 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   q.subset_nodes = tmp32;
   CK(up_raw(h, &tmp32, in->node_pod_off, (size_t)E + 1));
   q.node_pod_off = tmp32;
-  q.pod_class = h->cur->d_pod_class;
+  q.pod_class = cl.d_pod_class;
   q.n_extra = n_extra;
   q.extra_row0 = (int)extra_row0;
   if (n_extra > 0) {
@@ -1975,7 +1903,7 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   }
   q.deadline_ns = deadline_ms > 0 ? std::max<int64_t>(ms_left(), 1) * 1000000ll : 0;
   CK(zeros(h, &q.t_start, 1));
-  CK(zeros(h, &tmp32, (size_t)std::max<int64_t>(h->cur->P, 1)));
+  CK(zeros(h, &tmp32, (size_t)std::max<int64_t>(cl.P, 1)));
   int32_t* d_rank = tmp32;
   q.pod_rank = d_rank;
   {
@@ -1995,8 +1923,9 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   // ---- launch geometry: as many resident warps as the GPU holds, each with a private scratch slot
   const size_t budget = 200 * 1024;
   const size_t fixed = KP_ALIGN16(sizeof(ConsolShared));
-  size_t tb = plan_tables(h, fixed, budget);
-  size_t smem = fixed + tb + 64;
+  KpDev dq = d;  // the cluster's pointer block with k_consolidate's table plan (the upload keeps the solver's)
+  dq.tab_bytes = plan_tables(dq, fixed, budget);
+  const size_t smem = fixed + dq.tab_bytes + 64;
   const bool lean = !t.has_bounds && !t.min_values_strict && t.n_rsv == 0 && d.n_hostports == 0 && !getenv("KP_NO_LEAN");  // (G == 0 here)
   CK(cudaFuncSetAttribute(lean ? k_consolidate<true> : k_consolidate<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int per_sm = 1;
@@ -2067,7 +1996,7 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   CK(cudaMemsetAsync(q.decision, KP_DECISION_UNKNOWN, S1, h->stream));  // a subset the deadline cut off stays unknown
   CK(zeros(h, &q.next, 1));
   CK(zeros(h, &q.status, 1));
-  rc = reset_dynamic(h);
+  rc = reset_dynamic(h, cl);
   if (rc != KP_OK) return rc;
   auto t_up = std::chrono::steady_clock::now();
   h->stats.upload_ms += std::chrono::duration<double, std::milli>(t_up - t_begin).count();
@@ -2079,19 +2008,19 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
     k_feasibility<<<(d.N * 32 + 255) / 256, 256, 0, h->stream>>>(d, nullptr, 1);
     h->stats.kernel_launches++;
   }
-  rc = sort_queue(h);  // byCPUAndMemoryDescending over every pod row; a subset's queue is its rows in rank order
+  rc = sort_queue(h, cl);  // byCPUAndMemoryDescending over every pod row; a subset's queue is its rows in rank order
   if (rc != KP_OK) return rc;
-  if (h->cur->P > 0) {
-    k_scatter_rank<<<(int)((h->cur->P + 255) / 256), 256, 0, h->stream>>>(d.queue, h->cur->P, d_rank);
+  if (cl.P > 0) {
+    k_scatter_rank<<<(int)((cl.P + 255) / 256), 256, 0, h->stream>>>(d.queue, cl.P, d_rank);
     h->stats.kernel_launches++;
   }
-  rc = launch_node_cand(h);
+  rc = launch_node_cand(h, cl);
   if (rc != KP_OK) return rc;
   if (S > 0) {
     if (lean)
-      k_consolidate<true><<<grid, CONSOL_WARPS * 32, smem, h->stream>>>(d, q);
+      k_consolidate<true><<<grid, CONSOL_WARPS * 32, smem, h->stream>>>(dq, q);
     else
-      k_consolidate<false><<<grid, CONSOL_WARPS * 32, smem, h->stream>>>(d, q);
+      k_consolidate<false><<<grid, CONSOL_WARPS * 32, smem, h->stream>>>(dq, q);
     h->stats.kernel_launches++;
   }
   CK(cudaEventRecord(h->ev1, h->stream));
@@ -2105,38 +2034,9 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   if (status != KP_OK) return h->err = "consolidation instance failed (capacity or invalid state)", status;
   // ---- results
   auto t0 = std::chrono::steady_clock::now();
-  CK(cudaMemcpy(out->decision, q.decision, (size_t)S, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(out->replacement_its, q.replacement_its, (size_t)S * ITW * 8, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(out->n_new_claims, q.n_new_claims, (size_t)S * 4, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(out->n_unscheduled, q.n_unscheduled, (size_t)S * 4, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(out->repl_template, q.repl_tmpl, (size_t)S * 4, cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(out->repl_requests, q.repl_req, (size_t)S * R * 8, cudaMemcpyDeviceToHost));
-  {
-    std::vector<uint8_t> sfl((size_t)S1 * K);
-    std::vector<uint64_t> smk((size_t)S1 * K);
-    std::vector<int64_t> sg, sl;
-    CK(cudaMemcpy(sfl.data(), q.repl_sflags, (size_t)S * K, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(smk.data(), q.repl_smask, (size_t)S * K * 8, cudaMemcpyDeviceToHost));
-    if (t.has_bounds) {
-      sg.resize((size_t)S1 * K);
-      sl.resize((size_t)S1 * K);
-      CK(cudaMemcpy(sg.data(), q.repl_sgte, (size_t)S * K * 8, cudaMemcpyDeviceToHost));
-      CK(cudaMemcpy(sl.data(), q.repl_slte, (size_t)S * K * 8, cudaMemcpyDeviceToHost));
-    }
-    for (int s_ = 0; s_ < S; s_++)
-      if (out->decision[s_] == KP_DECISION_REPLACE)
-        store_repl(s_, sfl.data() + (size_t)s_ * K, smk.data() + (size_t)s_ * K, t.has_bounds ? sg.data() + (size_t)s_ * K : nullptr,
-                   t.has_bounds ? sl.data() + (size_t)s_ * K : nullptr);
-      else
-        out->repl_template[s_] = -1;
-  }
-  if (in->export_price_order) {
-    std::vector<int32_t> ord((size_t)S1 * order_cap), on(S1);
-    CK(cudaMemcpy(ord.data(), q.repl_order, (size_t)S * order_cap * 4, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(on.data(), q.repl_order_n, (size_t)S * 4, cudaMemcpyDeviceToHost));
-    for (int s_ = 0; s_ < S; s_++) order_rows[s_].assign(ord.begin() + (size_t)s_ * order_cap, ord.begin() + (size_t)s_ * order_cap + on[s_]);
-    finish_order();
-  }
+  rc = read_consol(h, q, S, nullptr, L, R, ITW, order_rows, out);
+  if (rc != KP_OK) return rc;
+  finish_order();
   out->solve_ms = ms;
   h->stats.bytes_d2h = (size_t)S * (13 + (size_t)ITW * 8 + (size_t)R * 8 + (size_t)K * 9);
   h->stats.download_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();

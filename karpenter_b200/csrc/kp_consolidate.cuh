@@ -2,7 +2,8 @@
 //
 //   k_node_cand     existing-node candidate bitmaps: for every (class signature | request vector) x node one bit.
 //                   Streams the node table once per signature tile -- the HBM-bound, embarrassingly parallel part.
-//   k_wsolve        Scheduler.Solve: one instance, one CTA; order / failure bitmaps / staged tables in shared memory.
+//   k_wsolve_batch  Scheduler.Solve: one CTA per instance (n >= 1); order / failure bitmaps / staged tables in shared
+//                   memory.
 //   k_consolidate   disruption.SimulateScheduling + computeConsolidation (helpers.go:51-142, consolidation.go:136-229)
 //                   for every candidate subset: one warp per subset pulled from a global counter, 8 warps per CTA, all
 //                   SMs busy; the cluster's node table is shared read-only, each warp keeps the nodes its simulation
@@ -274,13 +275,9 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CR) {
     d.counters[9] = I.fast_commits;
   }
 }
-template <bool LEAN, bool COHORT, bool VOL = false>
-__global__ void __launch_bounds__(64, 1) k_wsolve(const __grid_constant__ KpDev d_in, int CS, int CR) {
-  wsolve_cta<LEAN, COHORT, VOL>(d_in, CS, CR);
-}
-// Many Scheduler instances in one launch, one CTA (== one SM) each: NodePool shards of a provisioning pass, or the
-// candidate sets of a consolidation pass whose pods carry topology constraints (SimulateScheduling, helpers.go:51-142).
-// Instances share nothing but the device; plan[b] = {CS, CR} of instance b.
+// Scheduler instances in one launch, one CTA (== one SM) each: a single provisioning solve (a batch of one), NodePool
+// shards of a provisioning pass, or the candidate sets of a consolidation pass whose pods carry topology constraints
+// (SimulateScheduling, helpers.go:51-142).  Instances share nothing but the device; plan[b] = {CS, CR} of instance b.
 template <bool LEAN, bool COHORT, bool VOL = false>
 __global__ void __launch_bounds__(64, 1) k_wsolve_batch(const KpDev* __restrict__ devs, const int2* __restrict__ plan) {
   wsolve_cta<LEAN, COHORT, VOL>(devs[blockIdx.x], plan[blockIdx.x].x, plan[blockIdx.x].y);

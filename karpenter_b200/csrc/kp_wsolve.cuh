@@ -9,7 +9,7 @@
 //   lane w  owns word w of the instance-type bitmap
 //   lane i  owns candidate base+i while scanning the claim order / node bitmaps (ballot -> lowest index wins)
 //
-// The same routine serves the provisioning solve (one instance, k_wsolve) and the consolidation search (one instance
+// The same routine serves the provisioning solve (k_wsolve_batch) and the consolidation search (one instance
 // per removal subset, thousands of warps in flight, k_consolidate): an instance is a WInst, a block of pointers to
 // its private mutable state.  Existing nodes are found through per-class candidate bitmaps (supersets computed once
 // by k_node_cand) and every candidate is re-checked exactly; the consolidation instances share the cluster's base node
@@ -404,7 +404,7 @@ __device__ __forceinline__ void migrate_small(const KpDev& d, WInst& I, int nC, 
   __syncwarp();
 }
 
-// Pod staging ring between a stager warp and the solver warp of one CTA (k_wsolve): the stager walks the queue a few
+// Pod staging ring between a stager warp and the solver warp of one CTA (k_wsolve_batch): the stager walks the queue a few
 // pods ahead and parks each pod's class row (header, requests, requirement slots) in shared memory, so the solver's
 // dependence chain never waits on -- or spends instructions for -- the L2 loads of the next pod.
 #define KP_RING 8
