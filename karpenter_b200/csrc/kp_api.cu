@@ -7,7 +7,6 @@
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
-#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -412,174 +411,73 @@ static int upload_tables(kp_handle* h, Instance& in, const kp_problem* p, int cm
   CK(up(h, &d.mv_masks, t.mv_masks));
   CK(up(h, &d.cls_match, t.cls_match));
   CK(up(h, &d.cls_rec, t.cls_rec));
-  {  // class rows (one indirection less on the per-pod path)
-    std::vector<int32_t> hdr((size_t)std::max(t.X, 1) * KP_HDR, 0);
-    std::map<std::pair<int, int>, int> fsigs, nsigs;
-    std::vector<int32_t> nsig_rs, nsig_tolset;
-    std::vector<int4> hchk;
-    std::vector<uint64_t> tok(std::max(t.X, 1), 0);
-    size_t XK = (size_t)std::max(t.X, 1) * t.K;
-    std::vector<uint8_t> pf(XK, 0), sf(XK, 0);
-    std::vector<uint64_t> pm(XK, 0), sm(XK, 0);
-    std::vector<int64_t> pg(XK, 0), pl(XK, 0), sg(XK, 0), sl(XK, 0);
+  {  // class rows (one indirection less on the per-pod path): the class plan of kp_prep.cpp in the device's encoding
     if (t.N > 64) return h->err = "more than 64 NodePools", KP_ERR_CAPACITY;
-    // A key a NodeClaim does not define makes Compatible fail (requirements.go:181-197) until some pod with a NotIn /
-    // DoesNotExist requirement defines it -- the one way CanAdd can flip from false to true for a topology-free pod.
-    // It cannot happen for a row whose positive keys are all well-known (AllowUndefinedWellKnownLabels) or defined by
-    // every NodePool template; only such rows get a permanent failure bit.
-    auto row_monotone = [&](int rs) {
-      for (int k = 0; k < t.K; k++) {
-        size_t i = (size_t)rs * t.K + k;
-        Slot sl_{t.rs_flags[i], t.rs_mask[i], t.rs_gte[i], t.rs_lte[i]};
-        if (!slot_present(sl_) || op_is_negative(slot_op(sl_)) || t.key_wellknown[k]) continue;
-        for (int n = 0; n < t.N; n++)
-          if (!(t.rs_flags[(size_t)t.tmpl_rs[n] * t.K + k] & SF_PRESENT)) return false;
-      }
-      return true;
-    };
-    bool offerings_monotone = true;
-    for (int dd = 0; dd < t.D; dd++) offerings_monotone = offerings_monotone && row_monotone(t.offset_rs[dd]);
-    // can a pod ever define a new key on an existing node? (negative requirement on an undefined key, or a topology
-    // domain choice) -- if not, an undefined key fails the strict Compatible of existingnode.go:89 forever
-    bool nodes_gain_keys = false;
-    for (int g = 0; g < t.G; g++) nodes_gain_keys = nodes_gain_keys || t.groups[g].key != t.hostname_key;
-    // ---- the domain fast path (kp_kernels.cuh domain_mask): topology key = the non-hostname key most groups sit on
-    std::vector<int32_t> tkinfo(std::max(t.X, 1), 0xff);
-    {
-      std::vector<int> per_key(std::max(t.K, 1), 0);
-      for (int g = 0; g < t.G; g++)
-        if (t.groups[g].key != t.hostname_key && t.groups[g].key >= 0) per_key[t.groups[g].key]++;
-      d.tk_key = -1;
-      for (int k = 0; k < t.K; k++)
-        if (per_key[k] > 0 && (d.tk_key < 0 || per_key[k] > per_key[d.tk_key])) d.tk_key = k;
-      bool lazy = false;
-      for (int32_t b : t.g_born) lazy = lazy || b == 0;
-      const bool fp_global = !t.has_bounds && !lazy && !t.min_values_strict && t.n_rsv == 0 && !getenv("KP_NO_DOMAIN_FP");
-      // set inclusion of requirement slots without bounds: values(a) within values(b)
-      auto slot_subset = [&](int rs_a, int rs_b, int k) {
-        const size_t ia = (size_t)rs_a * t.K + k, ib = (size_t)rs_b * t.K + k;
-        const bool ac = t.rs_flags[ia] & SF_COMPLEMENT, bc = t.rs_flags[ib] & SF_COMPLEMENT;
-        const uint64_t am = t.rs_mask[ia], bm = t.rs_mask[ib];
-        if (!ac && !bc) return (am & ~bm) == 0;
-        if (!ac && bc) return (am & bm) == 0;
-        if (ac && bc) return (bm & ~am) == 0;
-        return false;
-      };
-      // TopologyNodeFilter.Matches (topologynodefilter.go:68-97) holds for every claim whose requirements the class's
-      // own requirement set leaves unchanged: some alternative is empty, or constrains only keys the class constrains
-      // at least as tightly
-      auto filter_implied = [&](int x, const KpGroup& G) {
-        for (int a = 0; a < G.filter_n; a++) {
-          const int rs = t.filter_rs[G.filter_off + a];
-          bool ok = true;
-          for (int k = 0; k < t.K && ok; k++) {
-            if (!(t.rs_flags[(size_t)rs * t.K + k] & SF_PRESENT)) continue;
-            ok = (t.rs_flags[(size_t)t.cls_rs[x] * t.K + k] & SF_PRESENT) && slot_subset(t.cls_rs[x], rs, k);
-          }
-          if (ok) return true;
-        }
-        return false;
-      };
-      std::map<int, int> asigs;
-      for (int x = 0; x < t.X; x++) {
-        auto it = asigs.find(t.cls_rs[x]);
-        if (it == asigs.end()) it = asigs.emplace(t.cls_rs[x], (int)asigs.size()).first;
-        int info = it->second < 64 ? it->second : 0xff;
-        const int nm = t.cls_match_off[x + 1] - t.cls_match_off[x], nr = t.cls_rec_off[x + 1] - t.cls_rec_off[x];
-        bool fp = fp_global && nm + nr > 0 && nm <= KP_PG && nr <= KP_PG, has_tk = false;
-        for (int i = t.cls_match_off[x]; i < t.cls_match_off[x + 1] && fp; i++) {
-          const KpGroup& G = t.groups[t.cls_match[i] & 0x3fffffff];
-          if (G.key == d.tk_key)
-            has_tk = true;
-          else if (G.key != t.hostname_key)
-            fp = false;
-        }
-        for (int i = t.cls_rec_off[x]; i < t.cls_rec_off[x + 1] && fp; i++) {
-          const KpGroup& G = t.groups[t.cls_rec[i]];
-          if (G.key == d.tk_key)
-            has_tk = true;
-          else if (G.key != t.hostname_key)
-            fp = false;
-          if (fp && !G.inverse && G.affinity_policy == 1 && G.filter_n > 0 && !filter_implied(x, G)) fp = false;
-        }
-        if (fp) info |= TKI_FP | (has_tk ? TKI_TK : 0);
-        if (it->second < 64) info |= TKI_ABIT;
-        if (nm + nr > 0) info |= TKI_TOPO;
-        tkinfo[x] = info;
-      }
-    }
-    // classes of a volume-alternative chain: the candidate loop tries the chain on every candidate, so nothing a single
-    // requirement set says about a candidate may be cached (signatures, shortcut flags), and every node is a candidate
-    std::vector<uint8_t> in_chain(std::max(t.X, 1), 0);
-    for (int x = 0; x < t.X; x++)
-      if (t.cls_vol_next[x] >= 0) in_chain[x] = in_chain[t.cls_vol_next[x]] = 1;
+    const ClassPlan& plan = t.plan;
+    const bool domain_fp = !getenv("KP_NO_DOMAIN_FP");
+    const size_t XK = (size_t)std::max(t.X, 1) * t.K;
+    std::vector<int64_t> pg(XK, 0), pl(XK, 0), sg(XK, 0), sl(XK, 0);
+    std::vector<ClsLane> rows((size_t)std::max(t.X, 1) * 32);
+    memset(rows.data(), 0, rows.size() * sizeof(ClsLane));
     for (int x = 0; x < t.X; x++) {
-      int32_t* hh = &hdr[(size_t)x * KP_HDR];
-      if (in_chain[x]) tkinfo[x] = 0xff;
-      hh[0] = t.cls_tolset[x];
-      hh[1] = t.cls_rv[x];
-      hh[2] = t.cls_match_off[x];
-      hh[3] = t.cls_match_off[x + 1];
-      hh[4] = t.cls_rec_off[x];
-      hh[5] = t.cls_rec_off[x + 1];
-      hh[6] = -1;
-      if (!in_chain[x] && t.cls_match_off[x + 1] == t.cls_match_off[x] && offerings_monotone && row_monotone(t.cls_rs[x])) {
-        auto key = std::make_pair(t.cls_rs[x], 0);  // failure bits record requirement incompatibility only
-        auto it = fsigs.find(key);
-        if (it == fsigs.end()) it = fsigs.emplace(key, (int)fsigs.size()).first;
-        hh[6] = it->second;
-        // the accepted-signature fast path: topology-free, counted by no group, nothing to re-check on the type list
-        if ((tkinfo[x] & TKI_ABIT) && t.cls_rec_off[x + 1] == t.cls_rec_off[x] && !t.min_values_strict && t.n_rsv == 0)
-          tkinfo[x] |= TKI_FAST;
+      // tkinfo: the accepted-signature id if it has a bit in amask, and the shortcuts; a chain class has neither
+      const int nm = t.cls_match_off[x + 1] - t.cls_match_off[x], nr = t.cls_rec_off[x + 1] - t.cls_rec_off[x];
+      const int asig = plan.asig[x];
+      int tki = 0xff;
+      if (!plan.chain[x]) {
+        tki = asig < 64 ? asig | TKI_ABIT : 0xff;
+        if (plan.fast[x] && asig < 64) tki |= TKI_FAST;
+        if (plan.fp[x] && nm <= KP_PG && nr <= KP_PG && domain_fp) tki |= TKI_FP | (plan.has_tk[x] ? TKI_TK : 0);
+        if (nm + nr > 0) tki |= TKI_TOPO;
       }
-      {
-        auto key = std::make_pair(in_chain[x] ? -1 : t.cls_rs[x], t.cls_tolset[x]);  // -1: tolerations only (k_node_cand)
-        auto it = nsigs.find(key);
-        if (it == nsigs.end()) {
-          it = nsigs.emplace(key, (int)nsigs.size()).first;
-          nsig_rs.push_back(key.first);
-          nsig_tolset.push_back(t.cls_tolset[x]);
+      const int32_t hdr[KP_HDR] = {t.cls_tolset[x], t.cls_rv[x], t.cls_match_off[x], t.cls_match_off[x + 1], t.cls_rec_off[x],
+                                   t.cls_rec_off[x + 1], plan.fsig[x], plan.nsig[x], plan.hchk_off[x], plan.hchk_off[x + 1]};
+      const size_t a = (size_t)t.cls_rs[x] * t.K, b = (size_t)t.cls_strict_rs[x] * t.K;
+      for (int l = 0; l < 32; l++) {
+        ClsLane& c = rows[(size_t)x * 32 + l];
+        if (l < t.K) {
+          c.pod_m = t.rs_mask[a + l];
+          c.strict_m = t.rs_mask[b + l];
+          c.pod_f = t.rs_flags[a + l];
+          c.strict_f = t.rs_flags[b + l];
+          pg[(size_t)x * t.K + l] = t.rs_gte[a + l];
+          pl[(size_t)x * t.K + l] = t.rs_lte[a + l];
+          sg[(size_t)x * t.K + l] = t.rs_gte[b + l];
+          sl[(size_t)x * t.K + l] = t.rs_lte[b + l];
         }
-        hh[7] = it->second;
-      }
-      hh[8] = (int)hchk.size();
-      for (int i = t.cls_match_off[x]; i < t.cls_match_off[x + 1]; i++) {
-        int e = t.cls_match[i], g = e & 0x3fffffff, self = (e >> 30) & 1;
-        const KpGroup& G = t.groups[g];
-        if (G.key == t.hostname_key) hchk.push_back(int4{G.host_row, G.type | (self << 8), G.max_skew, g});
-      }
-      hh[9] = (int)hchk.size();
-      for (int k = 0; k < t.K; k++) {
-        size_t i = (size_t)t.cls_rs[x] * t.K + k;
-        Slot sl_{t.rs_flags[i], t.rs_mask[i], t.rs_gte[i], t.rs_lte[i]};
-        if (slot_present(sl_) && op_is_negative(slot_op(sl_))) nodes_gain_keys = true;
-      }
-      for (int n = 0; n < t.N; n++) {
-        int ts = t.tmpl_taintset[n];
-        bool ok = ts < 0 || t.n_taintsets == 0 || t.tol_ok[(size_t)(t.cls_tolset[x] + 1) * t.n_taintsets + ts];
-        if (ok) tok[x] |= 1ull << n;
-      }
-      for (int k = 0; k < t.K; k++) {
-        size_t a = (size_t)t.cls_rs[x] * t.K + k, b = (size_t)t.cls_strict_rs[x] * t.K + k, o = (size_t)x * t.K + k;
-        pf[o] = t.rs_flags[a];
-        pm[o] = t.rs_mask[a];
-        pg[o] = t.rs_gte[a];
-        pl[o] = t.rs_lte[a];
-        sf[o] = t.rs_flags[b];
-        sm[o] = t.rs_mask[b];
-        sg[o] = t.rs_gte[b];
-        sl[o] = t.rs_lte[b];
+        if (l < t.R) c.req = t.cls_req[(size_t)x * t.R + l];
+        if (l < KP_HDR) c.hdr = hdr[l];
+        if (l == KP_HDR + 2) c.hdr = (int32_t)(plan.tok[x] & 0xffffffffull);
+        if (l == KP_HDR + 3) c.hdr = (int32_t)(plan.tok[x] >> 32);
+        if (l == KP_HDR + 4) c.hdr = t.cls_relax[x];
+        if (l == KP_HDR + 5) c.hdr = tki;
+        if (l == KP_HDR + 10) c.hdr = t.cls_vol_next[x];
+        if (l >= KP_HDR + 6 && l <= KP_HDR + 9 && p->n_hostports > 0 && p->class_hostports) {
+          const uint64_t ports = p->class_hostports[x];
+          uint64_t conf = 0;
+          for (uint64_t m = ports; m;) {
+            const int i = __builtin_ctzll(m);
+            m &= m - 1;
+            conf |= p->hostport_conflicts[i];
+          }
+          const uint64_t v = l < KP_HDR + 8 ? ports : conf;
+          c.hdr = (int32_t)(((l - KP_HDR) & 1) ? (v >> 32) : (v & 0xffffffffull));
+        }
       }
     }
-    d.n_fsig = (int)fsigs.size();
-    d.n_nsig = (int)nsigs.size();
-    d.EW = (t.E + 31) / 32;
-    in.strict_undefined = nodes_gain_keys ? 0 : 1;
+    std::vector<int4> hchk;
+    for (const HostCheck& c : plan.hchk) hchk.push_back(int4{c.row, c.type | (c.self << 8), c.max_skew, c.g});
     if (hchk.empty()) hchk.push_back(int4{0, 0, 0, 0});
+    std::vector<int32_t> nsig_rs = plan.nsig_rs, nsig_tolset = plan.nsig_tolset;
     if (nsig_rs.empty()) {
       nsig_rs.push_back(0);
       nsig_tolset.push_back(-1);
     }
+    d.tk_key = plan.tk_key;
+    d.n_fsig = plan.n_fsig;
+    d.n_nsig = (int)plan.nsig_rs.size();
+    d.EW = (t.E + 31) / 32;
+    in.strict_undefined = plan.strict_undefined ? 1 : 0;
     std::vector<int64_t> rv_req((size_t)std::max(t.n_rv, 1) * t.R, 0);
     for (int x = 0; x < t.X; x++)
       for (int r = 0; r < t.R; r++) rv_req[(size_t)t.cls_rv[x] * t.R + r] = t.cls_req[(size_t)x * t.R + r];
@@ -603,39 +501,7 @@ static int upload_tables(kp_handle* h, Instance& in, const kp_problem* p, int cm
     CK(zeros(h, &d.nstat_sum, (size_t)std::max(d.n_nsig, 1) * std::max(d.ESW, 1)));
     CK(zeros(h, &d.nfit, (size_t)std::max(t.n_rv, 1) * std::max(d.EW, 1)));
     CK(zeros(h, &d.nstat, (size_t)std::max(d.n_nsig, 1) * std::max(d.EW, 1)));
-    {
-      std::vector<ClsLane> rows((size_t)std::max(t.X, 1) * 32);
-      memset(rows.data(), 0, rows.size() * sizeof(ClsLane));
-      for (int x = 0; x < t.X; x++)
-        for (int l = 0; l < 32; l++) {
-          ClsLane& c = rows[(size_t)x * 32 + l];
-          if (l < t.K) {
-            c.pod_m = pm[(size_t)x * t.K + l];
-            c.strict_m = sm[(size_t)x * t.K + l];
-            c.pod_f = pf[(size_t)x * t.K + l];
-            c.strict_f = sf[(size_t)x * t.K + l];
-          }
-          if (l < t.R) c.req = t.cls_req[(size_t)x * t.R + l];
-          if (l < KP_HDR) c.hdr = hdr[(size_t)x * KP_HDR + l];
-          if (l == KP_HDR + 2) c.hdr = (int32_t)(tok[x] & 0xffffffffull);
-          if (l == KP_HDR + 3) c.hdr = (int32_t)(tok[x] >> 32);
-          if (l == KP_HDR + 4) c.hdr = t.cls_relax[x];
-          if (l == KP_HDR + 5) c.hdr = tkinfo[x];
-          if (l == KP_HDR + 10) c.hdr = t.cls_vol_next[x];
-          if (l >= KP_HDR + 6 && l <= KP_HDR + 9 && p->n_hostports > 0 && p->class_hostports) {
-            const uint64_t ports = p->class_hostports[x];
-            uint64_t conf = 0;
-            for (uint64_t m = ports; m;) {
-              const int i = __builtin_ctzll(m);
-              m &= m - 1;
-              conf |= p->hostport_conflicts[i];
-            }
-            const uint64_t v = l < KP_HDR + 8 ? ports : conf;
-            c.hdr = (int32_t)(((l - KP_HDR) & 1) ? (v >> 32) : (v & 0xffffffffull));
-          }
-        }
-      CK(up(h, &d.cls_lane, rows));
-    }
+    CK(up(h, &d.cls_lane, rows));
     CK(up(h, &d.cp_g, pg));
     CK(up(h, &d.cp_l, pl));
     CK(up(h, &d.cs_g, sg));
@@ -777,33 +643,6 @@ static int reset_dynamic(kp_handle* h, Instance& in) {
   return KP_OK;
 }
 
-// OrderByPrice lists: available offerings per instance type, cheapest first (types.go:238-257)
-struct PriceLists {
-  std::vector<int32_t> off, set;
-  std::vector<double> price;
-};
-static PriceLists order_by_price(const kp_problem* p, const HostTables& t) {
-  PriceLists l;
-  l.off.assign((size_t)p->n_its + 1, 0);
-  for (int ti = 0; ti < p->n_its; ti++) {
-    std::vector<std::pair<double, int>> ent;
-    for (int o = p->it_off_off[ti]; o < p->it_off_off[ti + 1]; o++)
-      if (p->off_available[o]) ent.push_back({p->off_price[o], t.off_set[o]});
-    std::stable_sort(ent.begin(), ent.end(),
-                     [](const std::pair<double, int>& a, const std::pair<double, int>& b) { return a.first < b.first; });
-    for (auto& e : ent) {
-      l.price.push_back(e.first);
-      l.set.push_back(e.second);
-    }
-    l.off[(size_t)ti + 1] = (int32_t)l.set.size();
-  }
-  if (l.set.empty()) {
-    l.set.push_back(0);
-    l.price.push_back(0);
-  }
-  return l;
-}
-
 // shared-memory bytes of the read-only tables a kernel stages next to `fixed` bytes of its own (0 = leave them in L2)
 static int plan_tables(const KpDev& d, size_t fixed, size_t budget) {
   const size_t tb = kp_tab_bytes(d);
@@ -902,19 +741,7 @@ static int add_instance(kp_handle* h, const kp_problem* p, int64_t cmax) {
   }
   CK(up_raw(h, &in.d_uid_hi, p->pod_uid_hi, P));
   CK(up_raw(h, &in.d_uid_lo, p->pod_uid_lo, P));
-  // class rank for byCPUAndMemoryDescending (queue.go:72-108): cpu desc, then memory desc
-  std::vector<int64_t> rank(std::max(in.host.X, 1), 0);
-  {
-    std::vector<int> idx(in.host.X);
-    for (int i = 0; i < in.host.X; i++) idx[i] = i;
-    auto key = [&](int x) { return std::make_pair(-in.host.cls_sort_cpu[x], -in.host.cls_sort_mem[x]); };
-    std::sort(idx.begin(), idx.end(), [&](int a, int b) { return key(a) < key(b); });
-    int64_t r = -1;
-    for (size_t i = 0; i < idx.size(); i++) {
-      if (i == 0 || key(idx[i]) != key(idx[i - 1])) r++;
-      rank[idx[i]] = r;
-    }
-  }
+  const std::vector<int64_t>& rank = in.host.plan.rank;  // byCPUAndMemoryDescending (queue.go:72-108)
   CK(up_raw(h, &in.d_class_rank, rank.data(), rank.size()));
   {
     // Pods of classes that are alone in their (cpu, memory) rank stand together in the queue (byCPUAndMemoryDescending, then
@@ -1647,63 +1474,7 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   };
   auto t_begin = std::chrono::steady_clock::now();
   // ---- host-side constants of the decision step
-  auto ki = [&](int k) { return KeyInfo{t.val_int.data() + (size_t)k * 64, t.val_isint[k], t.key_univ[k]}; };
-  auto rs_slot_h = [&](int rs, int k) {
-    size_t i = (size_t)rs * K + k;
-    return Slot{t.rs_flags[i], t.rs_mask[i], t.rs_gte[i], t.rs_lte[i]};
-  };
-  std::vector<double> node_price(std::max(E, 1), -1.0);  // getCandidatePrices (consolidation.go:319-337)
-  for (int n = 0; n < E; n++) {
-    int it = in->node_it[n];
-    if (it < 0) continue;
-    bool any = false;
-    double best = 0;
-    for (int o = p->it_off_off[it]; o < p->it_off_off[it + 1]; o++) {
-      bool ok = true;
-      for (int k = 0; k < K && ok; k++)
-        ok = slot_compatible(ki(k), rs_slot_h(p->node_reqset[n], k), rs_slot_h(p->off_reqset[o], k), t.key_wellknown[k], true);
-      if (!ok) continue;
-      if (!any || p->off_price[o] < best) best = p->off_price[o];
-      any = true;
-    }
-    if (any) node_price[n] = best;
-  }
-  const int ct_order[3] = {in->ct_reserved, in->ct_spot, in->ct_on_demand};
-  int ct_valid = 0;
-  std::vector<uint8_t> ctmask(std::max(t.D, 1), 0);
-  for (int i = 0; i < 3; i++) {
-    if (in->capacity_type_key < 0 || ct_order[i] < 0) continue;
-    ct_valid |= 1 << i;
-    for (int dd = 0; dd < t.D; dd++) {
-      bool ok = true;
-      for (int k = 0; k < K && ok; k++) {
-        Slot ex = k == in->capacity_type_key ? Slot{SF_PRESENT, 1ull << ct_order[i], 0, 0} : Slot{0u, 0ull, 0, 0};
-        ok = slot_compatible(ki(k), ex, t.off_slots[(size_t)dd * K + k], t.key_wellknown[k], true);
-      }
-      if (ok) ctmask[dd] |= 1 << i;
-    }
-  }
-  // WorstLaunchPrice lists (see KpConsol)
-  std::vector<int32_t> wl_off((size_t)T * 3 + 1, 0), wl_set;
-  std::vector<double> wl_price;
-  for (int ti = 0; ti < T; ti++)
-    for (int ci = 0; ci < 3; ci++) {
-      std::vector<std::pair<double, int>> ent;
-      for (int o = p->it_off_off[ti]; o < p->it_off_off[ti + 1]; o++)
-        if (p->off_available[o] && ((ctmask[t.off_set[o]] >> ci) & 1)) ent.push_back({p->off_price[o], t.off_set[o]});
-      std::stable_sort(ent.begin(), ent.end(), [](const std::pair<double, int>& a, const std::pair<double, int>& b) {
-        return a.first > b.first;
-      });
-      for (auto& e : ent) {
-        wl_price.push_back(e.first);
-        wl_set.push_back(e.second);
-      }
-      wl_off[(size_t)ti * 3 + ci + 1] = (int32_t)wl_set.size();
-    }
-  if (wl_set.empty()) {
-    wl_set.push_back(0);
-    wl_price.push_back(0);
-  }
+  const ConsolPrices cp = consol_prices(p, t, in);
   const PriceLists ml = order_by_price(p, t);
   // price tables and decision constants of the device side (both paths)
   auto upload_prices = [&](KpConsol& q) -> int {
@@ -1712,10 +1483,10 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
     q.ct_od = in->ct_on_demand;
     q.export_order = in->export_price_order ? 1 : 0;
     q.order_cap = order_cap;
-    q.ct_order_valid = ct_valid;
+    q.ct_order_valid = cp.ct_valid;
     q.spot_to_spot_enabled = in->spot_to_spot_enabled;
     q.T = T;
-    CK(up(h, &q.node_price, node_price));
+    CK(up(h, &q.node_price, cp.node_price));
     uint8_t* u8;
     CK(up_raw(h, &u8, in->node_is_spot, (size_t)E));
     q.node_is_spot = u8;
@@ -1726,9 +1497,9 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
     CK(up(h, &q.ml_off, ml.off));
     CK(up(h, &q.ml_set, ml.set));
     CK(up(h, &q.ml_price, ml.price));
-    CK(up(h, &q.wl_off, wl_off));
-    CK(up(h, &q.wl_set, wl_set));
-    CK(up(h, &q.wl_price, wl_price));
+    CK(up(h, &q.wl_off, cp.worst.off));
+    CK(up(h, &q.wl_set, cp.worst.set));
+    CK(up(h, &q.wl_price, cp.worst.price));
     CK(zeros(h, &q.sort_key, (size_t)std::max(T, 1)));  // one warp slot; the fast path re-allocates per slot below
     CK(zeros(h, &q.sort_val, (size_t)std::max(T, 1)));
     CK(zeros(h, &q.sort_bits, (size_t)std::max(ITW, 1)));

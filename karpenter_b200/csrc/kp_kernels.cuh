@@ -578,7 +578,7 @@ __device__ __forceinline__ void claims_finalize(const KpDev& d, uint8_t* sflags,
   __syncwarp();
 }
 
-// ---- the domain fast path (classes flagged TKI_FP, see upload_tables in kp_api.cu) -------------------------------
+// ---- the domain fast path (classes flagged TKI_FP, see plan_classes in kp_prep.cpp) ------------------------------
 // Every topology group of such a class sits on the hostname key or on ONE other key, the problem's "topology key" TK
 // (zone in practice).  A NodeClaim that already holds a pod is pinned to a single TK value z (its slot is In{z}); for
 // such a claim TopologyGroup.Get (topologygroup.go:226-428) answers either In{z} -- the claim's requirements stay as

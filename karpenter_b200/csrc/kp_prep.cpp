@@ -7,9 +7,9 @@ namespace {
 
 struct Ctx {
   const kp_problem* p;
-  HostTables& h;
+  const HostTables& h;
   int K, R;
-  Ctx(const kp_problem* pp, HostTables& hh) : p(pp), h(hh), K(pp->n_keys), R(pp->n_resources) {}
+  Ctx(const kp_problem* pp, const HostTables& hh) : p(pp), h(hh), K(pp->n_keys), R(pp->n_resources) {}
 
   KeyInfo ki(int k) const { return KeyInfo{h.val_int.data() + (size_t)k * 64, h.val_isint[k], h.key_univ[k]}; }
   Slot rs_slot(int rs, int k) const {
@@ -195,6 +195,148 @@ static int validate_problem(const kp_problem* p, std::string& err) {
   if (p->n_minvalue_keys > 0 && !csr(p->minvalue_it_off, (int64_t)p->n_minvalue_keys * p->n_its, -1)) KP_BAD("minvalue_it_off");
 #undef KP_BAD
   return KP_OK;
+}
+
+// ---- which shortcuts each class may take (ClassPlan), from the finished tables ----
+static void plan_classes(const Ctx& c, HostTables& h) {
+  const int K = h.K, N = h.N, X = h.X, X1 = std::max(X, 1);
+  ClassPlan& pl = h.plan;
+  pl = ClassPlan();
+  // A key a NodeClaim does not define makes Compatible fail (requirements.go:181-197) until some pod with a NotIn /
+  // DoesNotExist requirement defines it -- the one way CanAdd can flip from false to true for a topology-free pod.
+  // It cannot happen for a row whose positive keys are all well-known (AllowUndefinedWellKnownLabels) or defined by
+  // every NodePool template; only such rows get a permanent failure bit.
+  auto row_monotone = [&](int rs) {
+    for (int k = 0; k < K; k++) {
+      const Slot s = c.rs_slot(rs, k);
+      if (!slot_present(s) || op_is_negative(slot_op(s)) || h.key_wellknown[k]) continue;
+      for (int n = 0; n < N; n++)
+        if (!(h.rs_flags[(size_t)h.tmpl_rs[n] * K + k] & SF_PRESENT)) return false;
+    }
+    return true;
+  };
+  bool offerings_monotone = true;
+  for (int dd = 0; dd < h.D; dd++) offerings_monotone = offerings_monotone && row_monotone(h.offset_rs[dd]);
+  // set inclusion of requirement slots without bounds: values(a) within values(b)
+  auto slot_subset = [&](int rs_a, int rs_b, int k) {
+    const size_t ia = (size_t)rs_a * K + k, ib = (size_t)rs_b * K + k;
+    const bool ac = h.rs_flags[ia] & SF_COMPLEMENT, bc = h.rs_flags[ib] & SF_COMPLEMENT;
+    const uint64_t am = h.rs_mask[ia], bm = h.rs_mask[ib];
+    if (!ac && !bc) return (am & ~bm) == 0;
+    if (!ac && bc) return (am & bm) == 0;
+    if (ac && bc) return (bm & ~am) == 0;
+    return false;
+  };
+  // TopologyNodeFilter.Matches (topologynodefilter.go:68-97) holds for every claim whose requirements the class's
+  // own requirement set leaves unchanged: some alternative is empty, or constrains only keys the class constrains
+  // at least as tightly
+  auto filter_implied = [&](int x, const KpGroup& G) {
+    for (int a = 0; a < G.filter_n; a++) {
+      const int rs = h.filter_rs[G.filter_off + a];
+      bool ok = true;
+      for (int k = 0; k < K && ok; k++) {
+        if (!(h.rs_flags[(size_t)rs * K + k] & SF_PRESENT)) continue;
+        ok = (h.rs_flags[(size_t)h.cls_rs[x] * K + k] & SF_PRESENT) && slot_subset(h.cls_rs[x], rs, k);
+      }
+      if (ok) return true;
+    }
+    return false;
+  };
+  {  // the topology key of the domain fast path: the non-hostname key most groups sit on
+    std::vector<int> per_key(std::max(K, 1), 0);
+    for (int g = 0; g < h.G; g++)
+      if (h.groups[g].key != h.hostname_key && h.groups[g].key >= 0) per_key[h.groups[g].key]++;
+    for (int k = 0; k < K; k++)
+      if (per_key[k] > 0 && (pl.tk_key < 0 || per_key[k] > per_key[pl.tk_key])) pl.tk_key = k;
+  }
+  // can a pod ever define a new key on an existing node? (negative requirement on an undefined key, or a topology
+  // domain choice) -- if not, an undefined key fails the strict Compatible of existingnode.go:89 forever
+  bool nodes_gain_keys = false;
+  for (int g = 0; g < h.G; g++) nodes_gain_keys = nodes_gain_keys || h.groups[g].key != h.hostname_key;
+  for (int x = 0; x < X; x++)
+    for (int k = 0; k < K; k++) {
+      const Slot s = c.rs_slot(h.cls_rs[x], k);
+      if (slot_present(s) && op_is_negative(slot_op(s))) nodes_gain_keys = true;
+    }
+  pl.strict_undefined = !nodes_gain_keys;
+  // classes of a volume-alternative chain: the candidate loop tries the chain on every candidate, so nothing a single
+  // requirement set says about a candidate may be cached (signatures, shortcut flags), and every node is a candidate
+  pl.chain.assign(X1, 0);
+  for (int x = 0; x < X; x++)
+    if (h.cls_vol_next[x] >= 0) pl.chain[x] = pl.chain[h.cls_vol_next[x]] = 1;
+  // the domain fast path re-checks no bound, group birth, Strict minValues or reservation
+  bool lazy = false;
+  for (int32_t b : h.g_born) lazy = lazy || b == 0;
+  const bool fp_global = !h.has_bounds && !lazy && !h.min_values_strict && h.n_rsv == 0;
+  pl.fsig.assign(X1, -1);
+  pl.asig.assign(X1, 0);
+  pl.fast.assign(X1, 0);
+  pl.fp.assign(X1, 0);
+  pl.has_tk.assign(X1, 0);
+  pl.tok.assign(X1, 0);
+  pl.nsig.assign(X1, 0);
+  pl.rank.assign(X1, 0);
+  pl.hchk_off.assign(X + 1, 0);
+  std::map<int, int> fsigs, asigs;
+  std::map<std::pair<int, int>, int> nsigs;
+  for (int x = 0; x < X; x++) {
+    const int rs = h.cls_rs[x];
+    const int moff = h.cls_match_off[x], mend = h.cls_match_off[x + 1], roff = h.cls_rec_off[x], rend = h.cls_rec_off[x + 1];
+    pl.asig[x] = asigs.emplace(rs, (int)asigs.size()).first->second;
+    if (!pl.chain[x] && mend == moff && offerings_monotone && row_monotone(rs)) {
+      pl.fsig[x] = fsigs.emplace(rs, (int)fsigs.size()).first->second;  // failure bits record requirement incompatibility only
+      // the accepted-signature fast path: topology-free, counted by no group, nothing to re-check on the type list
+      pl.fast[x] = rend == roff && !h.min_values_strict && h.n_rsv == 0;
+    }
+    // the domain fast path: every group that constrains or counts the class sits on the hostname key or on tk_key, and
+    // none needs the node filter's requirement check at record time
+    bool fp = fp_global && !pl.chain[x] && mend + rend > moff + roff, has_tk = false;
+    for (int i = moff; i < mend && fp; i++) {
+      const KpGroup& G = h.groups[h.cls_match[i] & 0x3fffffff];
+      if (G.key == pl.tk_key)
+        has_tk = true;
+      else if (G.key != h.hostname_key)
+        fp = false;
+    }
+    for (int i = roff; i < rend && fp; i++) {
+      const KpGroup& G = h.groups[h.cls_rec[i]];
+      if (G.key == pl.tk_key)
+        has_tk = true;
+      else if (G.key != h.hostname_key)
+        fp = false;
+      if (fp && !G.inverse && G.affinity_policy == 1 && G.filter_n > 0 && !filter_implied(x, G)) fp = false;
+    }
+    pl.fp[x] = fp;
+    pl.has_tk[x] = fp && has_tk;
+    for (int n = 0; n < std::min(N, 64); n++) {
+      const int ts = h.tmpl_taintset[n];
+      if (ts < 0 || h.n_taintsets == 0 || h.tol_ok[(size_t)(h.cls_tolset[x] + 1) * h.n_taintsets + ts]) pl.tok[x] |= 1ull << n;
+    }
+    const auto key = std::make_pair(pl.chain[x] ? -1 : rs, h.cls_tolset[x]);
+    auto it = nsigs.find(key);
+    if (it == nsigs.end()) {
+      it = nsigs.emplace(key, (int)nsigs.size()).first;
+      pl.nsig_rs.push_back(key.first);
+      pl.nsig_tolset.push_back(key.second);
+    }
+    pl.nsig[x] = it->second;
+    for (int i = moff; i < mend; i++) {
+      const int e = h.cls_match[i], g = e & 0x3fffffff;
+      const KpGroup& G = h.groups[g];
+      if (G.key == h.hostname_key) pl.hchk.push_back(HostCheck{G.host_row, G.type, (e >> 30) & 1, G.max_skew, g});
+    }
+    pl.hchk_off[x + 1] = (int)pl.hchk.size();
+  }
+  pl.n_fsig = (int)fsigs.size();
+  pl.n_asig = (int)asigs.size();
+  std::vector<int> idx(X);
+  for (int x = 0; x < X; x++) idx[x] = x;
+  auto rank_key = [&](int x) { return std::make_pair(-h.cls_sort_cpu[x], -h.cls_sort_mem[x]); };
+  std::sort(idx.begin(), idx.end(), [&](int a, int b) { return rank_key(a) < rank_key(b); });
+  for (int i = 0, r = -1; i < X; i++) {
+    if (i == 0 || rank_key(idx[i]) != rank_key(idx[i - 1])) r++;
+    pl.rank[idx[i]] = r;
+  }
 }
 
 int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
@@ -950,5 +1092,76 @@ int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
   if (h.cls_match.empty()) h.cls_match.push_back(0);
   if (h.cls_rec.empty()) h.cls_rec.push_back(0);
   (void)host_to_node;
+  plan_classes(c, h);
   return KP_OK;
+}
+
+// ---- price lists ----
+// Appends one list: the available offerings o of instance type ti with keep(o), by price (stable: ties keep offering order)
+template <class Keep>
+static void add_list(PriceLists& l, const kp_problem* p, const HostTables& t, int ti, bool dearest_first, Keep keep) {
+  std::vector<std::pair<double, int>> ent;
+  for (int o = p->it_off_off[ti]; o < p->it_off_off[ti + 1]; o++)
+    if (p->off_available[o] && keep(o)) ent.push_back({p->off_price[o], t.off_set[o]});
+  std::stable_sort(ent.begin(), ent.end(), [&](const std::pair<double, int>& a, const std::pair<double, int>& b) {
+    return dearest_first ? a.first > b.first : a.first < b.first;
+  });
+  for (auto& e : ent) {
+    l.price.push_back(e.first);
+    l.set.push_back(e.second);
+  }
+  l.off.push_back((int32_t)l.set.size());
+}
+static void pad(PriceLists& l) {
+  if (l.set.empty()) {
+    l.set.push_back(0);
+    l.price.push_back(0);
+  }
+}
+
+PriceLists order_by_price(const kp_problem* p, const HostTables& t) {
+  PriceLists l;
+  l.off.assign(1, 0);
+  for (int ti = 0; ti < p->n_its; ti++) add_list(l, p, t, ti, false, [](int) { return true; });
+  pad(l);
+  return l;
+}
+
+ConsolPrices consol_prices(const kp_problem* p, const HostTables& t, const kp_consol_input* in) {
+  const Ctx c(p, t);
+  const int K = t.K;
+  ConsolPrices cp;
+  cp.node_price.assign(std::max(t.E, 1), -1.0);
+  for (int n = 0; n < t.E; n++) {
+    const int it = in->node_it[n];
+    if (it < 0) continue;
+    bool any = false;
+    double best = 0;
+    for (int o = p->it_off_off[it]; o < p->it_off_off[it + 1]; o++) {
+      if (!c.rows_compatible([&](int k) { return c.rs_slot(p->node_reqset[n], k); }, [&](int k) { return c.rs_slot(p->off_reqset[o], k); }, true))
+        continue;
+      if (!any || p->off_price[o] < best) best = p->off_price[o];
+      any = true;
+    }
+    if (any) cp.node_price[n] = best;
+  }
+  // bit i of a distinct offering set: compatible with capacity type i, in the order reserved, spot, on-demand
+  // (types.go:480-491)
+  const int ct_order[3] = {in->ct_reserved, in->ct_spot, in->ct_on_demand};
+  std::vector<uint8_t> ctmask(std::max(t.D, 1), 0);
+  for (int i = 0; i < 3; i++) {
+    if (in->capacity_type_key < 0 || ct_order[i] < 0) continue;
+    cp.ct_valid |= 1 << i;
+    const Slot ct{SF_PRESENT, 1ull << ct_order[i], 0, 0}, none{0u, 0ull, 0, 0};
+    for (int dd = 0; dd < t.D; dd++)
+      if (c.rows_compatible([&](int k) { return k == in->capacity_type_key ? ct : none; },
+                            [&](int k) { return t.off_slots[(size_t)dd * K + k]; }, true))
+        ctmask[dd] |= 1 << i;
+  }
+  cp.worst.off.assign(1, 0);
+  for (int ti = 0; ti < t.T; ti++)
+    for (int ci = 0; ci < 3; ci++)
+      add_list(cp.worst, p, t, ti, true, [&](int o) { return ((ctmask[t.off_set[o]] >> ci) & 1) != 0; });
+  pad(cp.worst);
+  return cp;
 }

@@ -2,8 +2,10 @@
 //
 // This is the part of scheduling.NewScheduler / NewTopology that runs once per Solve, not per pod
 // (scheduler.go:116-184, topology.go:68-143,162-194,297-426): requirement sets -> slot rows, taint toleration matrix,
-// bit-sliced instance-type tables, topology-group construction and initial domain counts.  The per-pod hot loop runs
-// on the device (kp_kernels.cu).
+// bit-sliced instance-type tables, topology-group construction and initial domain counts.  On top of these it decides
+// which shortcuts each class may take (ClassPlan) and builds the price lists of Results.TruncateInstanceTypes and
+// consolidation.  libkarpsolve.so encodes the result for the device, where the per-pod hot loop runs (kp_wsolve.cuh);
+// oracle/orc_cached.cpp runs the same algorithm over the same tables on one host core.
 #pragma once
 #include <algorithm>
 #include <cstring>
@@ -14,6 +16,33 @@
 
 #include "../../include/karpsolve.h"
 #include "kp_slot.hpp"
+
+// a hostname group among a class's match groups: a NodeClaim is exactly one hostname domain (next_candidate)
+struct HostCheck {
+  int row, type, self, max_skew, g;  // KpGroup::host_row, KpGroup::type, the class selects itself, KpGroup::max_skew, group
+};
+
+// Which shortcuts each class may take.  These decide exactness: a shortcut granted to the wrong class gives a wrong
+// answer.  Facts of the algorithm only; device limits (staging sizes, mask widths) are applied where they are encoded.
+struct ClassPlan {
+  int tk_key = -1;                // the topology key of the domain fast path: the non-hostname key most groups sit on
+  bool strict_undefined = false;  // no pod can define a new key on an existing node (k_node_cand)
+  int n_fsig = 0, n_asig = 0;
+  // per class [max(X, 1)]
+  std::vector<int32_t> fsig;    // failure signature, -1: none (a failed Compatible may not be permanent)
+  std::vector<int32_t> asig;    // accepted signature: id of the class's requirement set, in class order over all classes
+  std::vector<uint8_t> chain;   // member of a volume-alternative chain: no signature, no shortcut
+  std::vector<uint8_t> fast;    // the accepted-signature fast path: fsig >= 0, counted by no group, no re-check of the types
+  std::vector<uint8_t> fp;      // the domain fast path: every group on the hostname key or on tk_key, see plan_classes
+  std::vector<uint8_t> has_tk;  // fp and at least one group on tk_key
+  std::vector<uint64_t> tok;    // tolerated templates (the first 64)
+  std::vector<int32_t> nsig;    // existing-node signature: id of (requirement set, toleration set)
+  std::vector<int64_t> rank;    // NewQueue class rank: cpu desc, then memory desc (queue.go:72-108)
+  std::vector<int32_t> hchk_off;  // [X + 1] the class's hostname checks in hchk
+  std::vector<HostCheck> hchk;
+  // per existing-node signature: requirement set (-1: tolerations only, the chain classes) and toleration set
+  std::vector<int32_t> nsig_rs, nsig_tolset;
+};
 
 struct HostTables {
   int K = 0, R = 0, T = 0, ITW = 0, N = 0, X = 0, G = 0, GH = 0, E = 0, D = 0;
@@ -72,9 +101,27 @@ struct HostTables {
   std::vector<uint64_t> node_smask;
   std::vector<int64_t> node_sgte, node_slte;
   std::vector<int32_t> group_out_order;  // result order: regular groups (creation order) then inverse groups
+  ClassPlan plan;
 };
 
 // active: which nodes take part as existing nodes; extra_bound: additional (class,node) pods counted by the topology
 int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
                const std::vector<std::pair<int, int>>& extra_bound, const std::vector<int32_t>& pending_classes,
                HostTables& h, std::string& err);
+
+// Price lists of offerings: per list, a range [off[i], off[i + 1]) of (price, distinct offering set) entries.  `set` and
+// `price` are never empty, so each uploads as a table of at least one element.
+struct PriceLists {
+  std::vector<int32_t> off, set;
+  std::vector<double> price;
+};
+// OrderByPrice: available offerings per instance type, cheapest first (types.go:238-257)
+PriceLists order_by_price(const kp_problem* p, const HostTables& t);
+
+// The price tables of computeConsolidation (consolidation.go:136-337)
+struct ConsolPrices {
+  std::vector<double> node_price;  // [max(E, 1)] getCandidatePrices: the node's cheapest compatible offering, -1: none
+  int ct_valid = 0;                // bit i: capacity type i of (reserved, spot, on-demand) is known
+  PriceLists worst;                // WorstLaunchPrice: per (type, capacity type i) list 3 * type + i, dearest first
+};
+ConsolPrices consol_prices(const kp_problem* p, const HostTables& t, const kp_consol_input* in);

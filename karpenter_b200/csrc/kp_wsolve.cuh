@@ -1122,7 +1122,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
       sc.first_rclear = -1;
       sc.use_ez = false;
       sc.ez = ~0ull;
-      // tkinfo (host-computed per class, kp_api.cu upload_tables): which shortcuts the class may take
+      // tkinfo (host-computed per class, kp_prep.cpp plan_classes): which shortcuts the class may take
       const int tki = px.tkinfo;
       // bit of the pod's requirement set in the claims' "adds nothing" masks
       const unsigned long long abit = (tki & TKI_ABIT) ? 1ull << (tki & 63) : 0ull;

@@ -5,7 +5,7 @@
 // removes what that recomputes -- monotone failure bits per (claim, requirement signature / request vector), the
 // "adds nothing" fast path, threshold bitmaps instead of the per-type loop, scan lower bounds, the incremental form of Go's
 // sort.Slice -- and then walks the remaining chain with one warp.  This file walks the SAME chain with the SAME caches, over
-// the SAME prepared tables (kp_prep.cpp: the host half of libkarpsolve.so), as plain scalar C++: the ratio oracle : this
+// the SAME prepared tables and class plan (kp_prep.cpp: the host half of libkarpsolve.so), as plain scalar C++: the ratio oracle : this
 // is the algorithm's share of a speed-up, the ratio this : GPU the hardware's.
 //
 // Scope: Scheduler.Solve with existing nodes, in-flight and new NodeClaims -- requirement algebra without Gt / Lt bounds,
@@ -17,7 +17,6 @@
 #include <chrono>
 #include <cstdlib>
 #include <cstring>
-#include <map>
 #include <numeric>
 #include <string>
 #include <vector>
@@ -39,12 +38,9 @@ struct Claim {
 struct Solver {
   const kp_problem* p;
   HostTables t;
+  const ClassPlan& pl = t.plan;  // signatures and shortcuts per class (kp_prep.cpp plan_classes)
   int K, R, ITW, N, X;
-  std::vector<int> fsig, asig;  // per class: failure signature (-1: none), accepted signature
-  std::vector<uint8_t> fast;    // per class: may take the accepted-signature fast path (TKI_FAST)
-  std::vector<uint64_t> tok;    // per class: tolerated templates
   std::vector<uint64_t> tmpl_its;
-  int n_fsig = 0, n_asig = 0;
   std::vector<Claim> claims;
   std::vector<int32_t> ord;  // claim order (sort.Slice(newNodeClaims, len(Pods)))
   std::vector<int> cnt;      // pods per claim id
@@ -52,7 +48,7 @@ struct Solver {
   std::vector<int> lbf, lbr;                              // scan lower bounds per fsig / rv
   long long slow_sorts = 0, fast_commits = 0;
   // topology (kp_kernels.cuh): counters per group and domain, hostname groups counted per NodeClaim
-  int tk_key = -1, GH = 0;
+  int GH = 0;
   std::vector<int32_t> dom_cnt, g_ndomains, g_nempty;
   std::vector<uint64_t> dom_reg, dom_pop;
   std::vector<int32_t> host_cnt;            // [host * GH + row]; host = node index, or E + NodeClaim id
@@ -63,12 +59,8 @@ struct Solver {
   std::vector<uint32_t> node_rem_present;
   std::vector<Slot> node_slot;
   std::vector<int32_t> node_npods;
-  std::vector<int> nsig;                                // per class
   std::vector<std::vector<uint64_t>> nstat, nfit;       // bit per node
   std::vector<uint64_t> nactive;
-  std::vector<uint8_t> cls_fp, cls_tk;      // per class: domain fast path allowed (TKI_FP), has a topology-key group (TKI_TK)
-  struct HostCheck { int row, type, self, max_skew, g; };
-  std::vector<std::vector<HostCheck>> cls_hc;  // the hostname groups among a class's match groups
 
   KeyInfo ki(int k) const { return KeyInfo{t.val_int.data() + (size_t)k * 64, t.val_isint[k], t.key_univ[k]}; }
   Slot rs_slot(int rs, int k) const {
@@ -189,13 +181,13 @@ struct Solver {
   uint64_t domain_mask(int cls, bool* exact) const {
     uint64_t ez = ~0ull;
     *exact = true;
-    const Slot strict = rs_slot(t.cls_strict_rs[cls], tk_key);
-    const uint64_t univ = t.key_univ[tk_key];
+    const Slot strict = rs_slot(t.cls_strict_rs[cls], pl.tk_key);
+    const uint64_t univ = t.key_univ[pl.tk_key];
     const uint64_t pod_allowed = (strict.f & SF_PRESENT) ? (((strict.f & SF_COMPLEMENT) ? ~strict.m : strict.m) & univ) : univ;
     for (int i = t.cls_match_off[cls]; i < t.cls_match_off[cls + 1]; i++) {
       const int e = t.cls_match[i], g = e & 0x3fffffff;
       const KpGroup& G = t.groups[g];
-      if (G.key != tk_key) continue;
+      if (G.key != pl.tk_key) continue;
       const bool self = (e >> 30) & 1;
       const uint64_t reg = dom_reg[g], pop = dom_pop[g];
       if (G.type == KP_TOPO_SPREAD) {
@@ -386,91 +378,7 @@ struct Solver {
     for (int r = 0; r < GH; r++)
       for (int n = 0; n < E; n++) host_cnt[(size_t)n * GH + r] = t.host_cnt_nodes[(size_t)r * E + n];
     dom_cnt = t.dom_cnt, dom_reg = t.dom_reg, dom_pop = t.dom_pop, g_ndomains = t.g_ndomains, g_nempty = t.g_nempty;
-    {  // kp_api.cu upload_tables: the topology key = the non-hostname key most groups sit on
-      std::vector<int> per_key(std::max(K, 1), 0);
-      for (int g = 0; g < t.G; g++)
-        if (t.groups[g].key != t.hostname_key && t.groups[g].key >= 0) per_key[t.groups[g].key]++;
-      for (int k = 0; k < K; k++)
-        if (per_key[k] > 0 && (tk_key < 0 || per_key[k] > per_key[tk_key])) tk_key = k;
-    }
-    // kp_api.cu upload_tables: signatures and shortcut flags per class
-    auto row_monotone = [&](int rs) {
-      for (int k = 0; k < K; k++) {
-        const Slot sl = rs_slot(rs, k);
-        if (!slot_present(sl) || op_is_negative(slot_op(sl)) || t.key_wellknown[k]) continue;
-        for (int n = 0; n < N; n++)
-          if (!(t.rs_flags[(size_t)t.tmpl_rs[n] * K + k] & SF_PRESENT)) return false;
-      }
-      return true;
-    };
-    bool offerings_monotone = true;
-    for (int dd = 0; dd < t.D; dd++) offerings_monotone = offerings_monotone && row_monotone(t.offset_rs[dd]);
-    auto slot_subset = [&](int rs_a, int rs_b, int k) {
-      const size_t ia = (size_t)rs_a * K + k, ib = (size_t)rs_b * K + k;
-      const bool ac = t.rs_flags[ia] & SF_COMPLEMENT, bc = t.rs_flags[ib] & SF_COMPLEMENT;
-      const uint64_t am = t.rs_mask[ia], bm = t.rs_mask[ib];
-      if (!ac && !bc) return (am & ~bm) == 0;
-      if (!ac && bc) return (am & bm) == 0;
-      if (ac && bc) return (bm & ~am) == 0;
-      return false;
-    };
-    auto filter_implied = [&](int x, const KpGroup& G) {
-      for (int a = 0; a < G.filter_n; a++) {
-        const int rs = t.filter_rs[G.filter_off + a];
-        bool ok = true;
-        for (int k = 0; k < K && ok; k++) {
-          if (!(t.rs_flags[(size_t)rs * K + k] & SF_PRESENT)) continue;
-          ok = (t.rs_flags[(size_t)t.cls_rs[x] * K + k] & SF_PRESENT) && slot_subset(t.cls_rs[x], rs, k);
-        }
-        if (ok) return true;
-      }
-      return false;
-    };
-    fsig.assign(X, -1), asig.assign(X, 0), fast.assign(X, 0), tok.assign(X, 0);
-    cls_fp.assign(X, 0), cls_tk.assign(X, 0), cls_hc.assign(X, {});
-    std::map<int, int> fs, as;
-    for (int x = 0; x < X; x++) {
-      auto ia = as.find(t.cls_rs[x]);
-      if (ia == as.end()) ia = as.emplace(t.cls_rs[x], (int)as.size()).first;
-      asig[x] = ia->second;
-      {  // the domain fast path (TKI_FP): every group of the class on the hostname key or on the topology key
-        const int nm = t.cls_match_off[x + 1] - t.cls_match_off[x], nr = t.cls_rec_off[x + 1] - t.cls_rec_off[x];
-        bool fp = nm + nr > 0, has_tk = false;
-        for (int i = t.cls_match_off[x]; i < t.cls_match_off[x + 1] && fp; i++) {
-          const KpGroup& G = t.groups[t.cls_match[i] & 0x3fffffff];
-          if (G.key == tk_key)
-            has_tk = true;
-          else if (G.key != t.hostname_key)
-            fp = false;
-        }
-        for (int i = t.cls_rec_off[x]; i < t.cls_rec_off[x + 1] && fp; i++) {
-          const KpGroup& G = t.groups[t.cls_rec[i]];
-          if (G.key == tk_key)
-            has_tk = true;
-          else if (G.key != t.hostname_key)
-            fp = false;
-          if (fp && !G.inverse && G.affinity_policy == 1 && G.filter_n > 0 && !filter_implied(x, G)) fp = false;
-        }
-        cls_fp[x] = fp, cls_tk[x] = fp && has_tk;
-        for (int i = t.cls_match_off[x]; i < t.cls_match_off[x + 1]; i++) {
-          const int e = t.cls_match[i], g = e & 0x3fffffff;
-          const KpGroup& G = t.groups[g];
-          if (G.key == t.hostname_key) cls_hc[x].push_back(HostCheck{G.host_row, G.type, (e >> 30) & 1, G.max_skew, g});
-        }
-      }
-      if (t.cls_match_off[x + 1] == t.cls_match_off[x] && offerings_monotone && row_monotone(t.cls_rs[x])) {
-        auto it = fs.find(t.cls_rs[x]);
-        if (it == fs.end()) it = fs.emplace(t.cls_rs[x], (int)fs.size()).first;
-        fsig[x] = it->second;
-        fast[x] = t.cls_rec_off[x + 1] == t.cls_rec_off[x];  // (TKI_FAST: counted by no group either)
-      }
-      for (int n = 0; n < N; n++) {
-        const int ts = t.tmpl_taintset[n];
-        if (ts < 0 || t.n_taintsets == 0 || t.tol_ok[(size_t)(t.cls_tolset[x] + 1) * t.n_taintsets + ts]) tok[x] |= 1ull << n;
-      }
-    }
-    n_fsig = (int)fs.size(), n_asig = (int)as.size();
-    lbf.assign(std::max(n_fsig, 1), 0), lbr.assign(std::max(t.n_rv, 1), 0);
+    lbf.assign(std::max(pl.n_fsig, 1), 0), lbr.assign(std::max(t.n_rv, 1), 0);
     // k_feasibility, prefilter_only: NewScheduler keeps the template's types that pass its own requirements with zero
     // requests (scheduler.go:147)
     tmpl_its.assign((size_t)std::max(N, 1) * ITW, 0ull);
@@ -485,39 +393,24 @@ struct Solver {
       for (int i = 0; i < ITW; i++) tmpl_its[(size_t)n * ITW + i] = w[i] & t.tmpl_its_raw[(size_t)n * ITW + i];
     }
     // k_node_cand: candidate bitmaps of the existing nodes per (requirement set, toleration set) and per request vector
-    bool nodes_gain_keys = false;
-    for (int g = 0; g < t.G; g++) nodes_gain_keys = nodes_gain_keys || t.groups[g].key != t.hostname_key;
-    for (int x = 0; x < X; x++)
-      for (int k = 0; k < K; k++) {
-        const Slot sl = rs_slot(t.cls_rs[x], k);
-        if (slot_present(sl) && op_is_negative(slot_op(sl))) nodes_gain_keys = true;
-      }
-    const bool strict_undefined = !nodes_gain_keys;
-    nsig.assign(X, 0);
-    std::map<std::pair<int, int>, int> ns;
     const size_t ew = nactive.size();
-    for (int x = 0; x < X; x++) {
-      auto key = std::make_pair(t.cls_rs[x], t.cls_tolset[x]);
-      auto it = ns.find(key);
-      if (it == ns.end()) {
-        it = ns.emplace(key, (int)ns.size()).first;
-        nstat.emplace_back(ew, 0ull);
-        for (int n = 0; n < E; n++) {
-          bool ok = tolerated(t.cls_tolset[x], t.node_taintset[n]);
-          for (int k = 0; k < K && ok; k++) {
-            const Slot pod = rs_slot(t.cls_rs[x], k);
-            if (!slot_present(pod)) continue;
-            const Slot nd = node_slot[(size_t)n * K + k];
-            if (!slot_present(nd)) {
-              if (strict_undefined && !op_is_negative(slot_op(pod))) ok = false;
-            } else if (!slot_has_intersection(ki(k), nd, pod) && !(op_is_negative(slot_op(pod)) && op_is_negative(slot_op(nd)))) {
-              ok = false;
-            }
+    for (size_t s = 0; s < pl.nsig_rs.size(); s++) {
+      const int rs = pl.nsig_rs[s];
+      nstat.emplace_back(ew, 0ull);
+      for (int n = 0; n < E; n++) {
+        bool ok = tolerated(pl.nsig_tolset[s], t.node_taintset[n]);
+        for (int k = 0; k < K && ok; k++) {
+          const Slot pod = rs_slot(rs, k);
+          if (!slot_present(pod)) continue;
+          const Slot nd = node_slot[(size_t)n * K + k];
+          if (!slot_present(nd)) {
+            if (pl.strict_undefined && !op_is_negative(slot_op(pod))) ok = false;
+          } else if (!slot_has_intersection(ki(k), nd, pod) && !(op_is_negative(slot_op(pod)) && op_is_negative(slot_op(nd)))) {
+            ok = false;
           }
-          if (ok) set(nstat.back(), n);
         }
+        if (ok) set(nstat.back(), n);
       }
-      nsig[x] = it->second;
     }
     nfit.assign(std::max(t.n_rv, 1), std::vector<uint64_t>(ew, 0ull));
     std::vector<uint8_t> rv_done(std::max(t.n_rv, 1), 0);
@@ -540,22 +433,9 @@ struct Solver {
   }
 
   // NewQueue (queue.go:72-108): class rank by cpu desc, memory desc; then creation time, then UID
-  std::vector<int64_t> rank;
   void sort_rows(std::vector<int32_t>& rows) {
-    if (rank.empty()) {
-      rank.assign(std::max(X, 1), 0);
-      std::vector<int> idx(X);
-      std::iota(idx.begin(), idx.end(), 0);
-      auto key = [&](int x) { return std::make_pair(-t.cls_sort_cpu[x], -t.cls_sort_mem[x]); };
-      std::sort(idx.begin(), idx.end(), [&](int a, int b) { return key(a) < key(b); });
-      int64_t r = -1;
-      for (size_t i = 0; i < idx.size(); i++) {
-        if (i == 0 || key(idx[i]) != key(idx[i - 1])) r++;
-        rank[idx[i]] = r;
-      }
-    }
     std::stable_sort(rows.begin(), rows.end(), [&](int32_t a, int32_t b) {
-      const int64_t ra = rank[p->pod_class[a]], rb = rank[p->pod_class[b]];
+      const int64_t ra = pl.rank[p->pod_class[a]], rb = pl.rank[p->pod_class[b]];
       if (ra != rb) return ra < rb;
       const int64_t ta = p->pod_creation ? p->pod_creation[a] : 0, tb = p->pod_creation ? p->pod_creation[b] : 0;
       if (ta != tb) return ta < tb;
@@ -607,8 +487,8 @@ struct Solver {
     enum { PERT_NONE, PERT_INC, PERT_APPEND };
     int pert = PERT_NONE, pert_pos = 0;
     size_t head = 0;
-    const size_t fw = (size_t)(std::max(n_fsig, 1) + 63) / 64, rw = (size_t)(std::max(t.n_rv, 1) + 63) / 64,
-                 aw = (size_t)(std::max(n_asig, 1) + 63) / 64;
+    const size_t fw = (size_t)(std::max(pl.n_fsig, 1) + 63) / 64, rw = (size_t)(std::max(t.n_rv, 1) + 63) / 64,
+                 aw = (size_t)(std::max(pl.n_asig, 1) + 63) / 64;
     Eval ev;
     while (head < queue.size()) {
       // ---- Queue.Pop (queue.go:46-60)
@@ -616,12 +496,12 @@ struct Solver {
       const int32_t li = queue[head];
       if ((int64_t)head >= P && last_len[li] == len) break;  // a full cycle without progress
       head++;
-      const int cls = p->pod_class[rows[li]], rv = t.cls_rv[cls], fs = fsig[cls];
+      const int cls = p->pod_class[rows[li]], rv = t.cls_rv[cls], fs = pl.fsig[cls];
       const int nC = (int)claims.size();
       // ---- addToExistingNode (scheduler.go:520-555): the first node in order that passes
       if (E > 0) {
         bool placed = false;
-        const std::vector<uint64_t>&fitrow = nfit[rv], &strow = nstat[nsig[cls]];
+        const std::vector<uint64_t>&fitrow = nfit[rv], &strow = nstat[pl.nsig[cls]];
         for (size_t w = 0; w < nactive.size() && !placed; w++) {
           for (uint64_t bits = fitrow[w] & strow[w] & nactive[w]; bits && !placed; bits &= bits - 1) {
             const int node = (int)w * 64 + __builtin_ctzll(bits);
@@ -714,13 +594,13 @@ struct Solver {
       {
         const int lbf_ = fs >= 0 ? lbf[fs] : 0, lbr_ = lbr[rv];
         const int lb = std::max(lbf_, lbr_);
-        const bool scanned = (tok[cls] & tmpl_all) != 0;
+        const bool scanned = (pl.tok[cls] & tmpl_all) != 0;
         int first_clear = -1, first_rclear = -1;
         // the class's shortcuts (wsolve_run: tkinfo): topology-free fast path, or the domain fast path with its mask
         const bool topo = t.cls_match_off[cls + 1] > t.cls_match_off[cls] || t.cls_rec_off[cls + 1] > t.cls_rec_off[cls];
-        const bool fast_ok = fast[cls];
-        bool dom_fp = topo && cls_fp[cls], use_ez = false;
-        const bool has_tk = cls_tk[cls];
+        const bool fast_ok = pl.fast[cls];
+        bool dom_fp = topo && pl.fp[cls], use_ez = false;
+        const bool has_tk = pl.has_tk[cls];
         uint64_t ez = ~0ull;
         if (dom_fp && has_tk) {
           bool exact;
@@ -728,7 +608,6 @@ struct Solver {
           use_ez = exact;
           dom_fp = exact;
         }
-        const std::vector<HostCheck>& hcs = cls_hc[cls];
         for (int pos = lb; scanned && pos < nC && !found; pos++) {
           const int c = ord[pos];
           const bool fclear = fs < 0 || !bit(failm[c], fs), rclear = !bit(deadm[c], rv);
@@ -736,11 +615,12 @@ struct Solver {
           if (first_rclear < 0 && rclear) first_rclear = pos;
           if (!fclear || !rclear) continue;
           Claim& cl = claims[c];
-          if (!((tok[cls] >> cl.tmpl) & 1ull)) continue;
+          if (!((pl.tok[cls] >> cl.tmpl) & 1ull)) continue;
           if (use_ez && cl.dom != 0xff && !((ez >> cl.dom) & 1ull)) continue;  // pinned to a value the pod may not use
           {  // hostname groups: a NodeClaim is one hostname domain (next_candidate)
             bool pass = true;
-            for (const HostCheck& hc : hcs) {
+            for (int i = pl.hchk_off[cls]; i < pl.hchk_off[cls + 1]; i++) {
+              const HostCheck& hc = pl.hchk[i];
               const int hcnt = host_cnt[(size_t)(E + c) * GH + hc.row];
               if (hc.type == KP_TOPO_SPREAD)
                 pass = hcnt + hc.self <= hc.max_skew;
@@ -754,7 +634,7 @@ struct Solver {
           }
           int zdom = -1;
           bool fp = false;
-          if ((fast_ok || dom_fp) && bit(accm[c], asig[cls])) {
+          if ((fast_ok || dom_fp) && bit(accm[c], pl.asig[cls])) {
             fp = true;
             if (!fast_ok && has_tk) {
               zdom = cl.dom;
@@ -780,7 +660,7 @@ struct Solver {
             if (!fast_ok) topo_record_fast(cls, zdom, t.tmpl_taintset[cl.tmpl], E + c);
           } else {
             eval(cls, E + c, cl.s, cl.q, cl.its, cl.j, ev);
-            if (ev.pod_noop) set(accm[c], asig[cls]);
+            if (ev.pod_noop) set(accm[c], pl.asig[cls]);
             if (!ev.ok) {
               if (ev.res_dead) set(deadm[c], rv);
               if (ev.compat_fail && fs >= 0) set(failm[c], fs);
@@ -788,7 +668,7 @@ struct Solver {
             }
             if (ev.changed) {
               cl.s = ev.F;
-              if (tk_key >= 0) cl.dom = pinned(ev.F[tk_key]);
+              if (pl.tk_key >= 0) cl.dom = pinned(ev.F[pl.tk_key]);
             }
             cl.q = ev.q;
             cl.j = ev.j;
@@ -813,7 +693,7 @@ struct Solver {
         bool alive = false;
         for (uint64_t w : tw) alive = alive || w;
         if (!alive) continue;
-        if (!((tok[cls] >> n) & 1ull)) continue;
+        if (!((pl.tok[cls] >> n) & 1ull)) continue;
         std::vector<Slot> b(K);
         for (int k = 0; k < K; k++) b[k] = rs_slot(t.tmpl_rs[n], k);
         std::vector<int64_t> bq(t.tmpl_daemon.begin() + (size_t)n * R, t.tmpl_daemon.begin() + (size_t)(n + 1) * R);
@@ -821,7 +701,7 @@ struct Solver {
         if (!ev.ok) continue;
         Claim cl;
         cl.s = ev.F;
-        if (tk_key >= 0) cl.dom = pinned(ev.F[tk_key]);
+        if (pl.tk_key >= 0) cl.dom = pinned(ev.F[pl.tk_key]);
         cl.q = ev.q;
         cl.j = ev.j;
         cl.its = ev.its;
@@ -833,7 +713,7 @@ struct Solver {
         failm.emplace_back(fw, 0ull);
         deadm.emplace_back(rw, 0ull);
         accm.emplace_back(aw, 0ull);
-        if (ev.pod_noop) set(accm[cnew], asig[cls]);
+        if (ev.pod_noop) set(accm[cnew], pl.asig[cls]);
         if (GH > 0) {  // Topology.Register(hostname) (nodeclaim.go:213): every hostname group learns the new, empty domain
           host_cnt.resize((size_t)(E + cnew + 1) * GH, 0);
           for (int g = 0; g < t.G; g++)
@@ -919,74 +799,17 @@ struct Solver {
       err = "orc_cached: consolidation of topology-free candidate pods without extra pods only";
       return KP_ERR_UNSUPPORTED;
     }
-    const int T = t.T, S = in->n_subsets, ct_key = in->capacity_type_key;
-    auto full_slot = [&](int rs, int k) {
-      const size_t i = (size_t)rs * K + k;
-      return Slot{t.rs_flags[i], t.rs_mask[i], t.rs_gte[i], t.rs_lte[i]};
-    };
-    // getCandidatePrices (consolidation.go:319-337): the cheapest offering compatible with the node's labels
-    std::vector<double> node_price(std::max(E, 1), -1.0);
-    for (int n = 0; n < E; n++) {
-      const int it = in->node_it[n];
-      if (it < 0) continue;
-      bool any = false;
-      double best = 0;
-      for (int o = p->it_off_off[it]; o < p->it_off_off[it + 1]; o++) {
-        bool ok = true;
-        for (int k = 0; k < K && ok; k++)
-          ok = slot_compatible(ki(k), full_slot(p->node_reqset[n], k), full_slot(p->off_reqset[o], k), t.key_wellknown[k], true);
-        if (!ok) continue;
-        if (!any || p->off_price[o] < best) best = p->off_price[o];
-        any = true;
-      }
-      if (any) node_price[n] = best;
-    }
-    // WorstLaunchPrice lists per capacity type in the order reserved, spot, on-demand (types.go:480-491), OrderByPrice lists
-    const int ct_order[3] = {in->ct_reserved, in->ct_spot, in->ct_on_demand};
-    int ct_valid = 0;
-    std::vector<uint8_t> ctmask(std::max(t.D, 1), 0);
-    for (int i = 0; i < 3; i++) {
-      if (ct_key < 0 || ct_order[i] < 0) continue;
-      ct_valid |= 1 << i;
-      for (int dd = 0; dd < t.D; dd++) {
-        bool ok = true;
-        for (int k = 0; k < K && ok; k++) {
-          const Slot ex = k == ct_key ? Slot{SF_PRESENT, 1ull << ct_order[i], 0, 0} : Slot{0u, 0ull, 0, 0};
-          ok = slot_compatible(ki(k), ex, t.off_slots[(size_t)dd * K + k], t.key_wellknown[k], true);
-        }
-        if (ok) ctmask[dd] |= 1 << i;
-      }
-    }
-    std::vector<int32_t> wl_off((size_t)T * 3 + 1, 0), wl_set, ml_off((size_t)T + 1, 0), ml_set;
-    std::vector<double> wl_price, ml_price;
-    for (int ti = 0; ti < T; ti++) {
-      for (int ci = 0; ci < 3; ci++) {
-        std::vector<std::pair<double, int>> ent;
-        for (int o = p->it_off_off[ti]; o < p->it_off_off[ti + 1]; o++)
-          if (p->off_available[o] && ((ctmask[t.off_set[o]] >> ci) & 1)) ent.push_back({p->off_price[o], t.off_set[o]});
-        std::stable_sort(ent.begin(), ent.end(), [](const std::pair<double, int>& a, const std::pair<double, int>& b) { return a.first > b.first; });
-        for (auto& e : ent) {
-          wl_price.push_back(e.first);
-          wl_set.push_back(e.second);
-        }
-        wl_off[(size_t)ti * 3 + ci + 1] = (int32_t)wl_set.size();
-      }
-      std::vector<std::pair<double, int>> ent;
-      for (int o = p->it_off_off[ti]; o < p->it_off_off[ti + 1]; o++)
-        if (p->off_available[o]) ent.push_back({p->off_price[o], t.off_set[o]});
-      std::stable_sort(ent.begin(), ent.end(), [](const std::pair<double, int>& a, const std::pair<double, int>& b) { return a.first < b.first; });
-      for (auto& e : ent) {
-        ml_price.push_back(e.first);
-        ml_set.push_back(e.second);
-      }
-      ml_off[(size_t)ti + 1] = (int32_t)ml_set.size();
-    }
+    const int S = in->n_subsets, ct_key = in->capacity_type_key;
+    // getCandidatePrices, the WorstLaunchPrice lists per capacity type and the OrderByPrice lists (kp_prep.cpp)
+    const ConsolPrices cp = consol_prices(p, t, in);
+    const std::vector<double>& node_price = cp.node_price;
+    const PriceLists ml = order_by_price(p, t);
     const double INF = 1.7976931348623157e308;
     auto worst = [&](int ty, unsigned okmask) {
       for (int ci = 0; ci < 3; ci++) {
-        if (ct_key < 0 || !((ct_valid >> ci) & 1)) continue;
-        for (int e = wl_off[(size_t)ty * 3 + ci]; e < wl_off[(size_t)ty * 3 + ci + 1]; e++)
-          if ((okmask >> wl_set[e]) & 1u) return wl_price[e];
+        if (ct_key < 0 || !((cp.ct_valid >> ci) & 1)) continue;
+        for (int e = cp.worst.off[(size_t)ty * 3 + ci]; e < cp.worst.off[(size_t)ty * 3 + ci + 1]; e++)
+          if ((okmask >> cp.worst.set[e]) & 1u) return cp.worst.price[e];
       }
       return INF;
     };
@@ -1059,9 +882,9 @@ struct Solver {
             for (uint64_t b = cur[w]; b; b &= b - 1) {
               const int ty = w * 64 + __builtin_ctzll(b);
               double mp = INF;
-              for (int e = ml_off[ty]; e < ml_off[ty + 1]; e++)
-                if ((okmask >> ml_set[e]) & 1u) {
-                  mp = ml_price[e];
+              for (int e = ml.off[ty]; e < ml.off[ty + 1]; e++)
+                if ((okmask >> ml.set[e]) & 1u) {
+                  mp = ml.price[e];
                   break;
                 }
               types.push_back(ty);
@@ -1086,8 +909,8 @@ struct Solver {
               uint64_t keep = 0;
               for (uint64_t b = cur[w]; b; b &= b - 1) {
                 const int ty = w * 64 + __builtin_ctzll(b);
-                for (int e = ml_off[ty]; e < ml_off[ty + 1]; e++)
-                  if ((okmask >> ml_set[e]) & 1u) {
+                for (int e = ml.off[ty]; e < ml.off[ty + 1]; e++)
+                  if ((okmask >> ml.set[e]) & 1u) {
                     keep |= 1ull << (ty & 63);
                     break;
                   }
