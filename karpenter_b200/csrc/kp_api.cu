@@ -109,7 +109,7 @@ struct Instance {
   unsigned long long* trunc_bits = nullptr;
   uint8_t* d_dropped = nullptr;
   // shared-memory plan of the solve CTA (plan_solve)
-  int CS = 0, CR = 0;
+  int CS = 0, CQ = 0, CR = 0, tk_groups = 0;  // tk_groups: groups on the topology key whose state is on chip
   size_t smem = 0;
   // global counter table of a sharded job (kp_comm_set_counter_layout): dom_cnt index of each slot this instance owns
   int32_t* d_slot_src = nullptr;
@@ -162,7 +162,7 @@ struct kp_handle {
   enum Uploader { NONE, SINGLE, BATCH } uploaded = NONE;
   std::vector<std::unique_ptr<Instance>> insts;
   KpDev* d_devs = nullptr;  // [devs_cap] device copies of the instances' pointer blocks (run_solve)
-  int2* d_plan = nullptr;   // [devs_cap] {CS, CR}
+  int4* d_plan = nullptr;   // [devs_cap] {CS, CQ, CR, tk_groups}
   int devs_cap = 0;
   // sharded job: NCCL communicator + the global topology-domain counter table (device resident, all-reduced per solve)
   void* comm = nullptr;
@@ -512,6 +512,10 @@ static int upload_tables(kp_handle* h, Instance& in, const kp_problem* p, int cm
   CK(up_mut(h, in, &d.dom_cnt, t.dom_cnt));
   CK(up_mut(h, in, &d.dom_reg, t.dom_reg));
   CK(up_mut(h, in, &d.dom_pop, t.dom_pop));
+  d.tk_slot = nullptr;  // (on chip, set by k_wsolve_batch only)
+  d.tk_reg = d.tk_pop = nullptr;
+  d.tk_cnt = nullptr;
+  d.tk_nv = t.plan.tk_key >= 0 ? 64 - __builtin_clzll(t.key_univ[t.plan.tk_key] | 1ull) : 0;  // value ids lie below
   d.n_lazy = 0;
   for (int32_t b : t.g_born) d.n_lazy += b == 0;
   CK(up_mut(h, in, &d.g_born, t.g_born));
@@ -610,7 +614,7 @@ static int upload_tables(kp_handle* h, Instance& in, const kp_problem* p, int cm
     CK(up(h, &in.d_host_pop_nodes, bits));
   }
   CK(zeros(h, &d.n_claims, 1));
-  CK(zeros(h, &d.counters, 16));
+  CK(zeros(h, &d.counters, KP_NCOUNTERS));
   CK(zeros(h, &d.status, 1));
   return KP_OK;
 }
@@ -650,25 +654,50 @@ static int plan_tables(const KpDev& d, size_t fixed, size_t budget) {
 }
 
 // Host-side plan of the solver CTA; it depends on the upload and the KP_* knobs only.  Shared memory holds the pointer
-// block, the staged tables and, when they fit, the rows of the first CR claims and the claim order, template ids and
-// failure bitmaps of the first CS claims.
+// block, the staged tables and, when they fit, the hot claim rows of the first CQ claims, the cold ones of the first
+// CR <= CQ, and the claim order, template ids and failure bitmaps of the first CS claims.
 static void plan_solve(Instance& in) {
   KpDev& d = in.dev;
   const size_t budget = 224 * 1024;
   const size_t fixed = KP_ALIGN16(sizeof(WSolveShared));
   d.tab_bytes = plan_tables(d, fixed, budget);
   size_t tb = d.tab_bytes;
-  // rows of the first CR claims (requirement slots, requests, threshold rows, instance-type words) ...
-  auto row_bytes = [&](int cr) {
-    return KP_ALIGN16((size_t)cr * d.K * 8) + KP_ALIGN16((size_t)cr * d.R * 8) + KP_ALIGN16((size_t)cr * d.ITW * 8) +
-           KP_ALIGN16((size_t)cr * d.R * 4) + KP_ALIGN16((size_t)cr * d.K);
+  const bool dom_fp = std::any_of(in.host.plan.fp.begin(), in.host.plan.fp.end(), [](uint8_t f) { return f != 0; });
+  // The topology-key group state (every domain-fast-path pod reads it in domain_mask and writes it in topo_record_fast)
+  // goes first when it takes at most 64 KB: C3's 1 000 zone groups with 4 zones take 44 KB with the slot map.
+  in.tk_groups = 0;
+  if (dom_fp && !in.cohort && d.tk_key >= 0 && d.tk_nv > 0 && d.tk_nv <= 64) {
+    int ntk = 0;
+    for (const KpGroup& G : in.host.groups) ntk += G.key == d.tk_key;
+    if (ntk > 0 && kp_tk_bytes(d, ntk) <= 64 * 1024) {
+      in.tk_groups = ntk;
+      tb += kp_tk_bytes(d, ntk);
+    }
+  }
+  // claim rows (same layout as wsolve_cta): hot = requests + threshold row, cold = requirement slots + instance-type words
+  auto hot_bytes = [&](int n) { return KP_ALIGN16((size_t)n * d.R * 8) + KP_ALIGN16((size_t)n * d.R * 4); };
+  auto cold_bytes = [&](int n) {
+    return KP_ALIGN16((size_t)n * d.K * 8) + KP_ALIGN16((size_t)n * d.ITW * 8) + KP_ALIGN16((size_t)n * d.K);
   };
+  // The rows get what whole rows of up to 512 claims take within half the budget; the small arrays keep the rest.
   int CR = std::min(d.Cmax, 512);
-  while (CR > 0 && fixed + tb + row_bytes(CR) > budget / 2) CR -= 32;
+  while (CR > 0 && fixed + tb + hot_bytes(CR) + cold_bytes(CR) > budget / 2) CR -= 32;
   CR = std::max(CR, 0);
-  if (getenv("KP_CS_LIMIT")) CR = std::min(CR, 32);
-  if (const char* e = getenv("KP_CR")) CR = std::min(CR, std::max(0, atoi(e)) / 32 * 32);  // experiment knob
-  tb += CR ? row_bytes(CR) : 0;  // from here on `tb` is everything in front of the small arrays
+  const size_t rows = CR ? hot_bytes(CR) + cold_bytes(CR) : 0;
+  int CQ = CR;
+  // With classes on the domain fast path almost every commit is fp_fit + a store of the hot row: claims are visited
+  // round-robin, so the hot rows of as many claims as possible (C3: all of them) beat whole rows of a few hundred.
+  // Cold rows take what is left.
+  if (dom_fp) {
+    CQ = std::min((d.Cmax + 31) / 32 * 32, (int)(rows / ((size_t)d.R * 12 + 1)) / 32 * 32);
+    while (CQ > 0 && hot_bytes(CQ) > rows) CQ -= 32;
+    CR = 0;
+    while (CR + 32 <= CQ && hot_bytes(CQ) + cold_bytes(CR + 32) <= rows) CR += 32;
+  }
+  if (getenv("KP_CS_LIMIT")) CQ = std::min(CQ, 32);
+  if (const char* e = getenv("KP_CR")) CQ = std::min(CQ, std::max(0, atoi(e)) / 32 * 32);  // experiment knob: rows of <= n claims
+  CR = std::min(CR, CQ);
+  tb += (CQ ? hot_bytes(CQ) : 0) + (CR ? cold_bytes(CR) : 0);  // from here on `tb` is everything in front of the small arrays
   // ... and claim order / failure masks of the first CS claims
   auto small_bytes = [&](int cs) { return (size_t)cs * 37; };  // cmask 16 B + amask 8 B + order, count, template id, c_dom
   int CS = 0;
@@ -690,8 +719,12 @@ static void plan_solve(Instance& in) {
             !in.host.has_vol_alts && !getenv("KP_NO_LEAN");
   if (in.host.has_vol_alts) in.cohort = false;  // (the volume-alternative instantiation exists without cohorts only)
   in.CS = CS;
+  in.CQ = CQ;
   in.CR = CR;
   in.smem = fixed + tb + (CS ? small_bytes(CS) : 0) + 64;
+  if (getenv("KP_DEBUG"))
+    fprintf(stderr, "[kp] solver plan: tables %zu B, topology-key groups on chip %d, hot rows %d, cold rows %d, small arrays %d, %zu B shared\n",
+            (size_t)d.tab_bytes, in.tk_groups, CQ, CR, CS, in.smem);
 }
 
 // Starts a fresh upload: the instances of either entry point are dropped and the arena is reused for the new ones.
@@ -916,7 +949,7 @@ static const void* solver_kernel(const std::vector<std::unique_ptr<Instance>>& i
 }
 
 // Scheduler.Solve of every uploaded instance, a single solve being a batch of one.  In front of the timed window: the
-// dynamic state is restored and the pointer blocks and {CS, CR} plans are written to the device.  In it: the prep
+// dynamic state is restored and the pointer blocks and {CS, CQ, CR} plans are written to the device.  In it: the prep
 // kernels per instance, ONE solver launch (one CTA per instance), truncation and the counter all-reduce.
 // statuses[b]: KP_OK / KP_DEADLINE / KP_ERR_CAPACITY of instance b.
 static int run_solve(kp_handle* h, int64_t deadline_ms, std::vector<int32_t>& statuses) {
@@ -931,11 +964,11 @@ static int run_solve(kp_handle* h, int64_t deadline_ms, std::vector<int32_t>& st
     h->d_plan = nullptr;
     h->devs_cap = 0;
     CK(cudaMalloc(&h->d_devs, sizeof(KpDev) * n));
-    CK(cudaMalloc(&h->d_plan, sizeof(int2) * n));
+    CK(cudaMalloc(&h->d_plan, sizeof(int4) * n));
     h->devs_cap = n;
   }
   std::vector<KpDev> devs(n);
-  std::vector<int2> plan(n);
+  std::vector<int4> plan(n);
   size_t smem = 0;
   for (int b = 0; b < n; b++) {
     Instance& in = *h->insts[b];
@@ -944,11 +977,11 @@ static int run_solve(kp_handle* h, int64_t deadline_ms, std::vector<int32_t>& st
     int rc = reset_dynamic(h, in);
     if (rc != KP_OK) return rc;
     devs[b] = in.dev;
-    plan[b] = make_int2(in.CS, in.CR);
+    plan[b] = make_int4(in.CS, in.CQ, in.CR, in.tk_groups);
     smem = std::max(smem, in.smem);
   }
   CK(cudaMemcpyAsync(h->d_devs, devs.data(), sizeof(KpDev) * n, cudaMemcpyHostToDevice, h->stream));
-  CK(cudaMemcpyAsync(h->d_plan, plan.data(), sizeof(int2) * n, cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(h->d_plan, plan.data(), sizeof(int4) * n, cudaMemcpyHostToDevice, h->stream));
   CK(cudaEventRecord(h->ev0, h->stream));
   h->stats.kernel_launches = 0;
   h->stats.cohort_pods = 0;
@@ -1252,6 +1285,18 @@ int kp_comm_global_counts(kp_handle* h, int32_t* out, int64_t n) {
 }
 
 double kp_comm_last_allreduce_ms(kp_handle* h) { return h->allreduce_ms; }
+
+#ifdef KP_PHASE_PROF
+// Profiling build only: the solver warp's cycles per phase of the last solve of an instance (see KP_PROF_LAP), out[p] for
+// p < KP_NPHASE, then the cycles of the whole pod loop.  Returns the number of values written.
+int kp_phase_profile(kp_handle* h, int32_t instance, int64_t* out, int32_t n) {
+  Instance* in = pick_instance(h, instance);
+  if (!in || n < KP_NPHASE + 1) return h->err = "kp_phase_profile: no such instance or buffer too small", -1;
+  cudaSetDevice(h->device);
+  CK(cudaMemcpy(out, in->dev.counters + KP_PROF_AT, (KP_NPHASE + 1) * 8, cudaMemcpyDeviceToHost));
+  return KP_NPHASE + 1;
+}
+#endif
 
 void kp_comm_destroy(kp_handle* h) {
   if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);

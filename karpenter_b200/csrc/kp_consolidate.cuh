@@ -13,6 +13,12 @@
 
 #define KP_ALIGN16(x) (((x) + 15) & ~(size_t)15)
 
+// bytes of the state of the `ntk` groups on tk_key that a solver CTA keeps on chip (KpDev::tk_slot): the slot map, the
+// registered / populated masks and the counters with a stride of the key's value count (same formula on host and device)
+__host__ __device__ inline size_t kp_tk_bytes(const KpDev& d, int ntk) {
+  return KP_ALIGN16((size_t)d.G * 4) + 2 * KP_ALIGN16((size_t)ntk * 8) + KP_ALIGN16((size_t)ntk * d.tk_nv * 4);
+}
+
 // bytes of the read-only tables staged in shared memory (same formula on host and device)
 __host__ __device__ inline size_t kp_tab_bytes(const KpDev& d) {
   size_t K = d.K, R = d.R, ITW = d.ITW, D = d.D > 0 ? d.D : 1, N = d.N > 0 ? d.N : 1;
@@ -148,7 +154,7 @@ struct WSolveShared {
 
 // warp 0: the solver; warp 1: the pod stager (see StageRing)
 template <bool LEAN, bool COHORT, bool VOL>
-__device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CR) {
+__device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CQ, int CR, int ntk) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   WSolveShared& sh = *reinterpret_cast<WSolveShared*>(smem_raw);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -156,6 +162,34 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CR) {
   stage_tables(d_in, &sh.ds, tab);
   const KpDev& d = sh.ds;
   WInst& I = sh.inst;
+  unsigned char* p = tab + d_in.tab_bytes;
+  int32_t* s_slot = nullptr;
+  uint64_t *s_reg = nullptr, *s_pop = nullptr;
+  int32_t* s_cnt = nullptr;
+  if (ntk > 0) {  // the state of the groups on the topology key, numbered in group order (warp 0)
+    const int nv = d_in.tk_nv;
+    s_slot = reinterpret_cast<int32_t*>(p);
+    s_reg = reinterpret_cast<uint64_t*>(p + KP_ALIGN16((size_t)d_in.G * 4));
+    s_pop = s_reg + KP_ALIGN16((size_t)ntk * 8) / 8;
+    s_cnt = reinterpret_cast<int32_t*>(s_pop + KP_ALIGN16((size_t)ntk * 8) / 8);
+    if (warp == 0) {
+      for (int base = 0, n = 0; base < d_in.G; base += 32) {
+        const int g = base + lane;
+        const KpGroup* G_ = g < d_in.G ? d_in.groups + g : nullptr;
+        const bool on = G_ && G_->key == d_in.tk_key;
+        const unsigned m = __ballot_sync(FULL, on);
+        const int s = n + __popc(m & ((1u << lane) - 1));
+        if (g < d_in.G) s_slot[g] = on ? s : -1;
+        if (on) {
+          s_reg[s] = d_in.dom_reg[g];
+          s_pop[s] = d_in.dom_pop[g];
+          for (int v = 0; v < nv; v++) s_cnt[s * nv + v] = d_in.dom_cnt[G_->dom_off + v];
+        }
+        n += __popc(m);
+      }
+    }
+    p += kp_tk_bytes(d_in, ntk);
+  }
   const int Cmax = d.Cmax;
   if (threadIdx.x == 0) {
     sh.ring.produced = 0;
@@ -214,17 +248,26 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CR) {
     I.c_ports = d.c_ports;
     I.node_ports = d.node_ports;
     I.ov_ports = nullptr;
+    I.CQ = 0;
     I.CR = 0;
-    unsigned char* p = tab + d_in.tab_bytes;
-    if (CR > 0) {  // rows of the first CR claims
+    if (ntk > 0) {
+      sh.ds.tk_slot = s_slot;
+      sh.ds.tk_reg = s_reg;
+      sh.ds.tk_pop = s_pop;
+      sh.ds.tk_cnt = s_cnt;
+    }
+    if (CQ > 0) {  // hot rows of the first CQ claims (same formula as kp_api.cu plan_solve)
+      I.s_req = reinterpret_cast<int64_t*>(p);
+      p += KP_ALIGN16((size_t)CQ * d.R * 8);
+      I.s_j = reinterpret_cast<int32_t*>(p);
+      p += KP_ALIGN16((size_t)CQ * d.R * 4);
+      I.CQ = CQ;
+    }
+    if (CR > 0) {  // cold rows of the first CR claims
       I.s_smask = reinterpret_cast<uint64_t*>(p);
       p += KP_ALIGN16((size_t)CR * d.K * 8);
-      I.s_req = reinterpret_cast<int64_t*>(p);
-      p += KP_ALIGN16((size_t)CR * d.R * 8);
       I.s_its = reinterpret_cast<uint64_t*>(p);
       p += KP_ALIGN16((size_t)CR * d.ITW * 8);
-      I.s_j = reinterpret_cast<int32_t*>(p);
-      p += KP_ALIGN16((size_t)CR * d.R * 4);
       I.s_sflags = reinterpret_cast<uint8_t*>(p);
       p += KP_ALIGN16((size_t)CR * d.K);
       I.CR = CR;
@@ -252,6 +295,16 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CR) {
   wsolve_run<false, true, LEAN, COHORT, VOL>(d, I, sh.ring.slot[0], sh.scratch, lane, &sh.ring);
   const int nC = I.n_claims;
   claim_rows_flush(d, I, nC, lane);
+  if (ntk > 0) {  // before k_scatter_counts, the counter all-reduce and the download read them
+    for (int g = lane; g < d.G; g += 32) {
+      const int s = s_slot[g];
+      if (s < 0) continue;
+      d_in.dom_reg[g] = s_reg[s];
+      d_in.dom_pop[g] = s_pop[s];
+      for (int v = 0; v < d.tk_nv; v++) d_in.dom_cnt[d_in.groups[g].dom_off + v] = s_cnt[s * d.tk_nv + v];
+    }
+    __syncwarp();
+  }
   if (!LEAN) claims_finalize(d, I.c_sflags, I.c_smask, I.c_rsv, nC, lane);
   if (I.CS > 0) {  // the host reads the final order (claim_rank) and template ids from global memory
     for (int i = lane; i < nC; i += 32) {
@@ -273,14 +326,22 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CR) {
     d.counters[7] = I.n_unsched;
     d.counters[8] = I.n_uninit;
     d.counters[9] = I.fast_commits;
+#ifdef KP_PHASE_PROF
+    for (int p = 0; p < KP_NPHASE; p++) d.counters[KP_PROF_AT + p] = I.prof[p];
+    d.counters[KP_PROF_AT + KP_NPHASE] = I.prof_total;
+#endif
   }
 }
 // Scheduler instances in one launch, one CTA (== one SM) each: a single provisioning solve (a batch of one), NodePool
 // shards of a provisioning pass, or the candidate sets of a consolidation pass whose pods carry topology constraints
-// (SimulateScheduling, helpers.go:51-142).  Instances share nothing but the device; plan[b] = {CS, CR} of instance b.
+// (SimulateScheduling, helpers.go:51-142).  Instances share nothing but the device; plan[b] = {CS, CQ, CR, groups on the
+// topology key whose state is on chip (0: none)} of instance b.
 template <bool LEAN, bool COHORT, bool VOL = false>
-__global__ void __launch_bounds__(64, 1) k_wsolve_batch(const KpDev* __restrict__ devs, const int2* __restrict__ plan) {
-  wsolve_cta<LEAN, COHORT, VOL>(devs[blockIdx.x], plan[blockIdx.x].x, plan[blockIdx.x].y);
+__global__ void __launch_bounds__(64, 1) k_wsolve_batch(const KpDev* __restrict__ devs, const int4* __restrict__ plan) {
+  const int4 pl = plan[blockIdx.x];
+  // (the lean and cohort instantiations leave the topology-key state in global memory: the code to stage it costs their
+  // register allocation more than it saves)
+  wsolve_cta<LEAN, COHORT, VOL>(devs[blockIdx.x], pl.x, pl.y, pl.z, LEAN || COHORT ? 0 : pl.w);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -728,6 +789,7 @@ __global__ void __launch_bounds__(CONSOL_WARPS * 32, CONSOL_MIN_CTAS) k_consolid
     I.nfit_sum = d.nfit_sum;
     I.nstat_sum = d.nstat_sum;
     I.CS = 0;
+    I.CQ = 0;
     I.CR = 0;
     I.c_dom = nullptr;  // candidate sets with topology take the batch path (k_wsolve_batch)
     I.g_c_dom = nullptr;

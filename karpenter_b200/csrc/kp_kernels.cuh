@@ -128,13 +128,25 @@ __device__ __forceinline__ uint64_t filter_its_word(const KpDev& d, const Slot* 
   return compat_off_word(d, S, lane) & fw;
 }
 
+// Where the state of non-hostname group g lives: the on-chip copy of a group on the topology key while the solver CTA
+// keeps one (KpDev::tk_slot), else the global tables.
+struct GroupState {
+  uint64_t *reg, *pop;
+  int32_t* cnt;  // counter of value v at cnt[v]
+};
+__device__ __forceinline__ GroupState tk_state(const KpDev& d, int g, const KpGroup& G) {
+  const int s = (d.tk_slot && G.key == d.tk_key) ? d.tk_slot[g] : -1;
+  if (s >= 0) return GroupState{d.tk_reg + s, d.tk_pop + s, d.tk_cnt + s * d.tk_nv};
+  return GroupState{d.dom_reg + g, d.dom_pop + g, d.dom_cnt + G.dom_off};
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // TopologyGroup.Get for a non-hostname key (topologygroup.go:226-428). Runs on the lane that owns the key.
 // Returns the `domains` requirement; an empty concrete set means "no eligible domain".
 __device__ __forceinline__ Slot topo_domains(const KpDev& d, int g, const KpGroup& G, bool self, const Slot& pod_d,
                                              const Slot& node_d, uint64_t reg, uint64_t pop) {
   KeyInfo ki = key_info(d, G.key);
-  const int32_t* cnt = d.dom_cnt + G.dom_off;
+  const int32_t* cnt = tk_state(d, g, G).cnt;
   uint64_t pod_allowed = slot_allowed(ki, pod_d);
   uint64_t node_allowed = slot_allowed(ki, node_d);
   bool node_in = slot_present(node_d) && slot_op(node_d) == OP_IN;
@@ -332,7 +344,8 @@ __device__ __forceinline__ Eval eval_candidate(const KpDev& d, const PodCtx& px,
           if (!ok) fail = true;
         }
       } else if (lane == G.key) {
-        Slot dm = topo_domains(d, g, G, self, strict, M, d.dom_reg[g], d.dom_pop[g]);
+        const GroupState st = tk_state(d, g, G);
+        Slot dm = topo_domains(d, g, G, self, strict, M, *st.reg, *st.pop);
         if (dm.m == 0)
           fail = true;  // topologyError: domains.Len() == 0
         else
@@ -496,13 +509,14 @@ __device__ __forceinline__ void topo_record(const KpDev& d, const PodCtx& px, co
         else if (!(ff & SF_COMPLEMENT) && __popcll(mm) == 1)
           rec = mm;
         uint64_t bits = rec;
+        const GroupState st = tk_state(d, g, G);
         while (bits) {
           int v = __ffsll((long long)bits) - 1;
           bits &= bits - 1;
-          d.dom_cnt[G.dom_off + v]++;
+          st.cnt[v]++;
         }
-        d.dom_reg[g] |= rec;
-        d.dom_pop[g] |= rec;
+        *st.reg |= rec;
+        *st.pop |= rec;
       }
     }
   }
@@ -601,10 +615,11 @@ __device__ __forceinline__ uint64_t domain_mask(const KpDev& d, const PodCtx& px
     if (G.key != d.tk_key) continue;
     const int e = px.m_e[i], g = e & 0x3fffffff;
     const bool self = (e >> 30) & 1;
-    const uint64_t reg = d.dom_reg[g], pop = d.dom_pop[g];
+    const GroupState st = tk_state(d, g, G);
+    const uint64_t reg = *st.reg, pop = *st.pop;
     if (G.type == KP_TOPO_SPREAD) {
       // lane v (and v + 32) reads the counter of value v; min over the domains the pod may use (domainMinCount :289-310)
-      const int32_t* cnt = d.dom_cnt + G.dom_off;
+      const int32_t* cnt = st.cnt;
       const long long c0 = (reg >> lane) & 1ull ? (long long)cnt[lane] : 0, c1 = (reg >> (lane + 32)) & 1ull ? (long long)cnt[lane + 32] : 0;
       const uint64_t sup = reg & pod_allowed;
       long long mn = 2147483647LL;
@@ -643,10 +658,11 @@ __device__ __forceinline__ void topo_record_fast(const KpDev& d, const PodCtx& p
       if (G.key == d.hostname_key) {
         host_record(d, G.host_row, g, host);
       } else if (z >= 0) {
-        d.dom_cnt[G.dom_off + z]++;
+        const GroupState st = tk_state(d, g, G);
+        st.cnt[z]++;
         const uint64_t bit = 1ull << z;
-        if (!(d.dom_reg[g] & bit)) d.dom_reg[g] |= bit;
-        if (!(d.dom_pop[g] & bit)) d.dom_pop[g] |= bit;
+        if (!(*st.reg & bit)) *st.reg |= bit;
+        if (!(*st.pop & bit)) *st.pop |= bit;
       }
     }
   }

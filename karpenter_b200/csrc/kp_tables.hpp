@@ -144,6 +144,13 @@ struct KpDev {
   int32_t* dom_cnt;               // [sum over non-hostname groups of 64]
   uint64_t* dom_reg;              // [G] registered-domain mask (t.domains keys)
   uint64_t* dom_pop;              // [G] domains with count > 0 (complement of t.emptyDomains within dom_reg)
+  // Null, or while a k_wsolve_batch CTA keeps them on chip: the state of the groups on tk_key.  tk_slot[g] = index s of
+  // group g among them (-1: other key); its registered / populated masks are tk_reg[s] / tk_pop[s], its counter of
+  // value v is tk_cnt[s * tk_nv + v].  Every reader and writer goes through tk_state (kp_kernels.cuh).
+  int32_t* tk_slot;
+  uint64_t *tk_reg, *tk_pop;
+  int32_t* tk_cnt;
+  int tk_nv;                      // value ids of tk_key lie below this
   int32_t* g_ndomains;            // [G] hostname groups: len(t.domains)
   int32_t* g_nempty;              // [G] hostname groups: len(t.emptyDomains)
   int32_t* host_cnt;              // [H * GHS] HOST-major (existing nodes then claims), GHS = max(GH, 1) ints per host: only

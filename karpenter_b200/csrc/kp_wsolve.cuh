@@ -20,6 +20,26 @@
 
 enum { PERT_NONE = 0, PERT_INC = 1, PERT_APPEND = 2 };
 
+// Per-phase cycle profile of the solver warp (profiling build only: make libkarpsolve_prof.so, tools/phase_profile.py).
+// KP_PROF_LAP(p) charges the SM cycles since the previous lap to phase p, so the phases add up to the loop's cycles.
+// In the default build the macro is empty and WInst has no profile fields: the generated code is unchanged.
+enum { PH_POP = 0, PH_SORT, PH_DMASK, PH_SCAN, PH_FAST, PH_RECORD, PH_EVAL, PH_NEW, PH_OTHER, KP_NPHASE };
+#ifdef KP_PHASE_PROF
+#define KP_PROF_LAP(p)                        \
+  do {                                        \
+    const long long t_ = clock64();           \
+    if (lane == 0) I.prof[p] += t_ - prof_t;  \
+    prof_t = t_;                              \
+  } while (0)
+#define KP_PROF_AT 16  // KpDev::counters[KP_PROF_AT + p]: cycles of phase p, then the loop's total
+#define KP_NCOUNTERS (KP_PROF_AT + KP_NPHASE + 1)
+#else
+#define KP_PROF_LAP(p) \
+  do {                 \
+  } while (0)
+#define KP_NCOUNTERS 16
+#endif
+
 struct WInst {
   // pods: local ids 0..P-1
   int P;
@@ -38,8 +58,10 @@ struct WInst {
   int64_t *c_sgte, *c_slte;
   uint64_t* c_its;
   int32_t* c_j;             // [Cmax*R] threshold row of the claim's requests per resource (fits_word)
-  // rows of the first CR claims are kept in shared memory (0 = none); copied out when the solve ends
-  int CR;
+  // Claim rows kept in shared memory, copied out when the solve ends.  The hot part (requests, threshold row), which
+  // every commit reads and writes, for the first CQ claims; the cold part (requirement slots, instance-type words), which
+  // only full evaluations and threshold advances touch, for the first CR <= CQ.  0 = none.
+  int CQ, CR;
   uint8_t* s_sflags;
   uint64_t* s_smask;
   int64_t* s_req;
@@ -93,6 +115,9 @@ struct WInst {
   // results
   int n_claims, n_unsched, n_uninit, status;
   long long ev_existing, ev_inflight, ev_tmpl, commits, slow_sorts, scan_chunks, evals, fast_commits;
+#ifdef KP_PHASE_PROF
+  long long prof[KP_NPHASE], prof_total;  // cycles per phase / of the whole pod loop
+#endif
 };
 
 // index of `node` in the overlay, -1 if it is untouched (warp-uniform result)
@@ -119,21 +144,22 @@ __device__ __forceinline__ void claim_load(const KpDev& d, const WInst& I, int c
       b->f = I.s_sflags[c * K + lane];
       b->m = I.s_smask[c * K + lane];
     }
-    if (lane < R) {
-      *q = I.s_req[c * R + lane];
-      *j = I.s_j[c * R + lane];
-    }
     if (lane < ITW) *its = I.s_its[c * ITW + lane];
   } else {
     if (lane < K) {
       b->f = I.c_sflags[(size_t)c * K + lane];
       b->m = I.c_smask[(size_t)c * K + lane];
     }
-    if (lane < R) {
+    if (lane < ITW) *its = I.c_its[(size_t)c * ITW + lane];
+  }
+  if (lane < R) {
+    if (c < I.CQ) {
+      *q = I.s_req[c * R + lane];
+      *j = I.s_j[c * R + lane];
+    } else {
       *q = I.c_req[(size_t)c * R + lane];
       *j = I.c_j[(size_t)c * R + lane];
     }
-    if (lane < ITW) *its = I.c_its[(size_t)c * ITW + lane];
   }
   if (!LEAN && d.has_bounds && lane < K) {
     b->gte = I.c_sgte[(size_t)c * K + lane];
@@ -150,21 +176,22 @@ __device__ __forceinline__ void claim_store(const KpDev& d, WInst& I, int c, int
       I.s_sflags[c * K + lane] = (uint8_t)ev.F.f;
       I.s_smask[c * K + lane] = ev.F.m;
     }
-    if (lane < R) {
-      I.s_req[c * R + lane] = ev.q;
-      I.s_j[c * R + lane] = ev.j;
-    }
     if (lane < ITW) I.s_its[c * ITW + lane] = ev.its;
   } else {
     if (slots && lane < K) {
       I.c_sflags[(size_t)c * K + lane] = (uint8_t)ev.F.f;
       I.c_smask[(size_t)c * K + lane] = ev.F.m;
     }
-    if (lane < R) {
+    if (lane < ITW) I.c_its[(size_t)c * ITW + lane] = ev.its;
+  }
+  if (lane < R) {
+    if (c < I.CQ) {
+      I.s_req[c * R + lane] = ev.q;
+      I.s_j[c * R + lane] = ev.j;
+    } else {
       I.c_req[(size_t)c * R + lane] = ev.q;
       I.c_j[(size_t)c * R + lane] = ev.j;
     }
-    if (lane < ITW) I.c_its[(size_t)c * ITW + lane] = ev.its;
   }
   if (!LEAN && slots && d.has_bounds && lane < K) {
     I.c_sgte[(size_t)c * K + lane] = ev.F.gte;
@@ -176,7 +203,7 @@ __device__ __forceinline__ void claim_load_rq(const KpDev& d, const WInst& I, in
   *q = 0;
   *j = 0;
   if (lane < d.R) {
-    if (c < I.CR) {
+    if (c < I.CQ) {
       *q = I.s_req[c * d.R + lane];
       *j = I.s_j[c * d.R + lane];
     } else {
@@ -191,28 +218,30 @@ __device__ __forceinline__ uint64_t claim_load_its(const KpDev& d, const WInst& 
 }
 __device__ __forceinline__ void claim_store_rq(const KpDev& d, WInst& I, int c, int lane, int64_t q, int j, bool with_its,
                                                uint64_t its) {
-  if (c < I.CR) {
-    if (lane < d.R) {
+  if (lane < d.R) {
+    if (c < I.CQ) {
       I.s_req[c * d.R + lane] = q;
       I.s_j[c * d.R + lane] = j;
-    }
-    if (with_its && lane < d.ITW) I.s_its[c * d.ITW + lane] = its;
-  } else {
-    if (lane < d.R) {
+    } else {
       I.c_req[(size_t)c * d.R + lane] = q;
       I.c_j[(size_t)c * d.R + lane] = j;
     }
-    if (with_its && lane < d.ITW) I.c_its[(size_t)c * d.ITW + lane] = its;
+  }
+  if (with_its && lane < d.ITW) {
+    if (c < I.CR)
+      I.s_its[c * d.ITW + lane] = its;
+    else
+      I.c_its[(size_t)c * d.ITW + lane] = its;
   }
 }
 // copy the shared-memory claim rows to their global arrays (end of the solve)
 __device__ __forceinline__ void claim_rows_flush(const KpDev& d, WInst& I, int nC, int lane) {
-  const int n = nC < I.CR ? nC : I.CR;
+  const int n = nC < I.CR ? nC : I.CR, nq = nC < I.CQ ? nC : I.CQ;
   for (int i = lane; i < n * d.K; i += 32) {
     I.c_sflags[i] = I.s_sflags[i];
     I.c_smask[i] = I.s_smask[i];
   }
-  for (int i = lane; i < n * d.R; i += 32) {
+  for (int i = lane; i < nq * d.R; i += 32) {
     I.c_req[i] = I.s_req[i];
     I.c_j[i] = I.s_j[i];
   }
@@ -474,7 +503,8 @@ __device__ void stager_run(const KpDev& d, const WInst& I, StageRing* ring, cons
       }
       __syncwarp();
       // pull what the solver will read for this pod into L1 now: the presence rows of its hostname groups (the part
-      // that covers the NodeClaims: 8 lines == 8 192 claims) and the counter rows of its topology-key groups
+      // that covers the NodeClaims: 8 lines == 8 192 claims) and, unless they are on chip, the counter rows of its
+      // topology-key groups
       if (slot.n_hc > 0) {
         const int g8 = lane >> 3, l8 = lane & 7;  // four groups at a time, eight lines each
         for (int k = g8; k < slot.n_hc; k += 4) {
@@ -482,7 +512,7 @@ __device__ void stager_run(const KpDev& d, const WInst& I, StageRing* ring, cons
           if (w < d.HW) prefetch_l1(d.host_pop + (size_t)slot.hc[k].x * d.HW + w);
         }
       }
-      if (slot.n_mg > 0 && lane < 2 * slot.n_mg) {
+      if (!d.tk_slot && slot.n_mg > 0 && lane < 2 * slot.n_mg) {
         const KpGroup& G = slot.mg[lane >> 1];
         if (G.key == d.tk_key) prefetch_l1(d.dom_cnt + G.dom_off + (lane & 1) * 32);
       }
@@ -804,7 +834,14 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
   long long watchdog = 0;
   unsigned long long t_start = 0;
   if (d.deadline_ns > 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_start));
+#ifdef KP_PHASE_PROF
+  long long prof_t = clock64();
+  const long long prof_t0 = prof_t;
+  if (lane == 0)
+    for (int p = 0; p < KP_NPHASE; p++) I.prof[p] = 0;
+#endif
   for (;;) {
+    KP_PROF_LAP(PH_OTHER);
     // ---- Queue.Pop (queue.go:46-60)
     const int len = tail - head;
     if (len == 0) break;
@@ -879,6 +916,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
     const unsigned long long fbit = (fsig >= 0 && fsig < 64) ? 1ull << fsig : 0ull;
     const unsigned long long rbit = (rv < 64 && !(VOL && px.vol_next >= 0)) ? 1ull << rv : 0ull;
     bool found = false;
+    KP_PROF_LAP(PH_POP);
 
     // ================= addToExistingNode (scheduler.go:520-555) =================
     if (E > 0 && px.nsig >= 0) {
@@ -1021,6 +1059,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
     }
 
     // ================= sort.Slice(newNodeClaims, len(Pods) asc) (scheduler.go:504) =================
+    KP_PROF_LAP(PH_OTHER);
     if (pert != PERT_NONE) {
       const int p = pert_pos;
       const bool inversion = pert == PERT_INC ? (p + 1 < nC && cnt[p + 1] < cnt[p]) : (nC >= 2 && cnt[nC - 1] < cnt[nC - 2]);
@@ -1110,6 +1149,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
       }
       pert = PERT_NONE;
     }
+    KP_PROF_LAP(PH_SORT);
 
     // ================= addToInflightNode (scheduler.go:557-589) =================
     {
@@ -1154,6 +1194,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
         sc.hoff = 0;
         sc.hend = 0;
       }
+      KP_PROF_LAP(PH_DMASK);
       int lbf = 0, lbr = 0;
       if (fbit) lbf = __shfl_sync(FULL, fsig < 32 ? lb0 : lb1, fsig & 31);
       if (rbit) lbr = __shfl_sync(FULL, rv < 32 ? lr0 : lr1, rv & 31);
@@ -1179,12 +1220,14 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
         } else {
           cpos = next_candidate<1, LEAN>(d, I, ord, nC, from, sc, lane, E, &cc);
         }
+        KP_PROF_LAP(PH_SCAN);
         if (cpos < 0) break;
         from = cpos + 1;
         {
           if (!LEAN && px.port_conf && (I.c_ports[cc] & px.port_conf)) continue;  // host ports (nodeclaim.go:120-124)
           if (COHORT && coh_ok) {
             const CohortOut co = cohort_try<LEAN>(d, I, px, sc, ord, cnt, nC, lb, cpos, cc, E, lane, abit, rbit, fast_ok, has_tk);
+            KP_PROF_LAP(PH_FAST);
             evals += co.nevals;
             if (co.state == 2) {
               fast_commits += co.npods;
@@ -1222,6 +1265,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
             if (!ok) {  // nothing left that holds the merged requests: permanent for this request vector
               if (lane == 0) I.cmask[cc].y |= rbit;
               __syncwarp();
+              KP_PROF_LAP(PH_FAST);
               continue;
             }
             claim_store_rq(d, I, cc, lane, q, lo, any_adv, its);
@@ -1233,9 +1277,11 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
                 I.pod_error[li] = KP_PODERR_NONE;
               }
             }
+            KP_PROF_LAP(PH_FAST);
             if (!LEAN && !fast_ok) topo_record_fast(d, px, zdom, d.tmpl_taintset[I.c_tmpl[cc]], E + cc, lane);
             fast_commits++;
             __syncwarp();
+            KP_PROF_LAP(PH_RECORD);
             pert = PERT_INC;
             pert_pos = cpos;
             ev_inflight += cpos + 1;
@@ -1282,6 +1328,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
               I.cmask[cc] = mk;
             }
             __syncwarp();
+            KP_PROF_LAP(PH_EVAL);
             continue;
           }
           // NodeClaim.Add (nodeclaim.go:207-219)
@@ -1298,8 +1345,10 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
               I.pod_error[li] = KP_PODERR_NONE;
             }
           }
+          KP_PROF_LAP(PH_EVAL);
           if (!LEAN) topo_record(d, px, ev.F, d.tmpl_taintset[I.c_tmpl[cc]], E + cc, true, lane);
           __syncwarp();
+          KP_PROF_LAP(PH_RECORD);
           pert = PERT_INC;
           pert_pos = cpos;
           ev_inflight += cpos + 1;  // claims 0..cpos were evaluated by the reference
@@ -1482,6 +1531,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
       found = true;
       commits++;
     }
+    KP_PROF_LAP(PH_NEW);
     if (status != KP_OK) break;
     if (!found) {
       const int nx = err == KP_PODERR_RESERVED ? -1 : px.relax;  // staged with the class row: cls_relax[Xc]
@@ -1523,6 +1573,10 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
       __syncwarp();
     }
   }
+#ifdef KP_PHASE_PROF
+  KP_PROF_LAP(PH_OTHER);
+  if (lane == 0) I.prof_total = prof_t - prof_t0;
+#endif
   if (STAGED) {
     __syncwarp();
     if (lane == 0) ring->done = 1;
