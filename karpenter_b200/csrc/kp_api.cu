@@ -653,15 +653,14 @@ static int plan_tables(const KpDev& d, size_t fixed, size_t budget) {
   return (fixed + tb <= budget && tb <= 110 * 1024) ? (int)tb : 0;
 }
 
-// Host-side plan of the solver CTA; it depends on the upload and the KP_* knobs only.  Shared memory holds the pointer
-// block, the staged tables and, when they fit, the hot claim rows of the first CQ claims, the cold ones of the first
-// CR <= CQ, and the claim order, template ids and failure bitmaps of the first CS claims.
+// Host-side plan of the solver CTA; it depends on the upload and the KP_* knobs only.  Shared memory (SolveSmem) holds
+// the pointer block, the staged tables and, when they fit, the hot claim rows of the first CQ claims, the cold ones of
+// the first CR <= CQ, and the claim order, template ids and failure bitmaps of the first CS claims.
 static void plan_solve(Instance& in) {
   KpDev& d = in.dev;
   const size_t budget = 224 * 1024;
-  const size_t fixed = KP_ALIGN16(sizeof(WSolveShared));
-  d.tab_bytes = plan_tables(d, fixed, budget);
-  size_t tb = d.tab_bytes;
+  d.tab_bytes = plan_tables(d, SolveSmem(d, 0, 0, 0, 0, 0).tab, budget);
+  auto layout = [&](int CS, int CQ, int CR) { return SolveSmem(d, d.tab_bytes, CS, CQ, CR, in.tk_groups); };
   const bool dom_fp = std::any_of(in.host.plan.fp.begin(), in.host.plan.fp.end(), [](uint8_t f) { return f != 0; });
   // The topology-key group state (every domain-fast-path pod reads it in domain_mask and writes it in topo_record_fast)
   // goes first when it takes at most 64 KB: C3's 1 000 zone groups with 4 zones take 44 KB with the slot map.
@@ -669,45 +668,36 @@ static void plan_solve(Instance& in) {
   if (dom_fp && !in.cohort && d.tk_key >= 0 && d.tk_nv > 0 && d.tk_nv <= 64) {
     int ntk = 0;
     for (const KpGroup& G : in.host.groups) ntk += G.key == d.tk_key;
-    if (ntk > 0 && kp_tk_bytes(d, ntk) <= 64 * 1024) {
-      in.tk_groups = ntk;
-      tb += kp_tk_bytes(d, ntk);
-    }
+    const SolveSmem L(d, d.tab_bytes, 0, 0, 0, ntk);
+    if (ntk > 0 && L.s_req - L.tk_slot <= 64 * 1024) in.tk_groups = ntk;
   }
-  // claim rows (same layout as wsolve_cta): hot = requests + threshold row, cold = requirement slots + instance-type words
-  auto hot_bytes = [&](int n) { return KP_ALIGN16((size_t)n * d.R * 8) + KP_ALIGN16((size_t)n * d.R * 4); };
-  auto cold_bytes = [&](int n) {
-    return KP_ALIGN16((size_t)n * d.K * 8) + KP_ALIGN16((size_t)n * d.ITW * 8) + KP_ALIGN16((size_t)n * d.K);
-  };
-  // The rows get what whole rows of up to 512 claims take within half the budget; the small arrays keep the rest.
+  // claim rows: hot = requests + threshold row, cold = requirement slots + instance-type words.  The rows get what whole
+  // rows of up to 512 claims take within half the budget; the small arrays keep the rest.
   int CR = std::min(d.Cmax, 512);
-  while (CR > 0 && fixed + tb + hot_bytes(CR) + cold_bytes(CR) > budget / 2) CR -= 32;
+  while (CR > 0 && layout(0, CR, CR).cmask > budget / 2) CR -= 32;
   CR = std::max(CR, 0);
-  const size_t rows = CR ? hot_bytes(CR) + cold_bytes(CR) : 0;
+  const SolveSmem whole = layout(0, CR, CR);
+  const size_t rows = whole.cmask - whole.s_req;
   int CQ = CR;
   // With classes on the domain fast path almost every commit is fp_fit + a store of the hot row: claims are visited
   // round-robin, so the hot rows of as many claims as possible (C3: all of them) beat whole rows of a few hundred.
   // Cold rows take what is left.
   if (dom_fp) {
     CQ = std::min((d.Cmax + 31) / 32 * 32, (int)(rows / ((size_t)d.R * 12 + 1)) / 32 * 32);
-    while (CQ > 0 && hot_bytes(CQ) > rows) CQ -= 32;
+    while (CQ > 0 && layout(0, CQ, 0).cmask - whole.s_req > rows) CQ -= 32;
     CR = 0;
-    while (CR + 32 <= CQ && hot_bytes(CQ) + cold_bytes(CR + 32) <= rows) CR += 32;
+    while (CR + 32 <= CQ && layout(0, CQ, CR + 32).cmask - whole.s_req <= rows) CR += 32;
   }
   if (getenv("KP_CS_LIMIT")) CQ = std::min(CQ, 32);
-  if (const char* e = getenv("KP_CR")) CQ = std::min(CQ, std::max(0, atoi(e)) / 32 * 32);  // experiment knob: rows of <= n claims
   CR = std::min(CR, CQ);
-  tb += (CQ ? hot_bytes(CQ) : 0) + (CR ? cold_bytes(CR) : 0);  // from here on `tb` is everything in front of the small arrays
   // ... and claim order / failure masks of the first CS claims
-  auto small_bytes = [&](int cs) { return (size_t)cs * 37; };  // cmask 16 B + amask 8 B + order, count, template id, c_dom
   int CS = 0;
-  if (fixed + tb + small_bytes(64) + 64 <= budget) {  // the largest multiple of 32 that fits, capped at Cmax
+  if (layout(64, CQ, CR).total <= budget) {  // the largest multiple of 32 that fits, capped at Cmax
     int lo = 64, hi = ((d.Cmax + 31) / 32) * 32;
-    if (const char* e = getenv("KP_CS_CAP")) hi = std::min(hi, std::max(64, atoi(e) / 32 * 32));  // experiment knob
     while (lo < hi) {
       int mid = ((lo + hi + 32) / 64) * 32;
       if (mid <= lo) mid = lo + 32;
-      if (fixed + tb + small_bytes(mid) + 64 <= budget)
+      if (layout(mid, CQ, CR).total <= budget)
         lo = mid;
       else
         hi = mid - 32;
@@ -721,7 +711,7 @@ static void plan_solve(Instance& in) {
   in.CS = CS;
   in.CQ = CQ;
   in.CR = CR;
-  in.smem = fixed + tb + (CS ? small_bytes(CS) : 0) + 64;
+  in.smem = layout(CS, CQ, CR).total;
   if (getenv("KP_DEBUG"))
     fprintf(stderr, "[kp] solver plan: tables %zu B, topology-key groups on chip %d, hot rows %d, cold rows %d, small arrays %d, %zu B shared\n",
             (size_t)d.tab_bytes, in.tk_groups, CQ, CR, CS, in.smem);
@@ -1473,7 +1463,7 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
     h->err = "consolidation with minValues under the BestEffort policy is not supported yet";
     return KP_ERR_UNSUPPORTED;
   }
-  const int K = t.K, R = t.R, ITW = t.ITW, E = t.E, N = t.N, T = t.T;
+  const int K = t.K, R = t.R, ITW = t.ITW, E = t.E, T = t.T;
   const bool general = t.G > 0;  // the evicted pods carry topology constraints: one full solve per candidate set
   const ReqLayout L(cl);
   // ---- result arrays (owned by `out` from here on: kp_consolidate frees them on any error return)
@@ -1545,11 +1535,31 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
     CK(up(h, &q.wl_off, cp.worst.off));
     CK(up(h, &q.wl_set, cp.worst.set));
     CK(up(h, &q.wl_price, cp.worst.price));
-    CK(zeros(h, &q.sort_key, (size_t)std::max(T, 1)));  // one warp slot; the fast path re-allocates per slot below
-    CK(zeros(h, &q.sort_val, (size_t)std::max(T, 1)));
-    CK(zeros(h, &q.sort_bits, (size_t)std::max(ITW, 1)));
     return KP_OK;
   };
+  // per-row outputs of `n` candidate sets
+  auto alloc_rows = [&](KpConsol& q, size_t n) -> int {
+    CK(zeros(h, &q.decision, n));
+    CK(zeros(h, &q.replacement_its, n * std::max(ITW, 1)));
+    CK(zeros(h, &q.n_new_claims, n));
+    CK(zeros(h, &q.n_unscheduled, n));
+    CK(zeros(h, &q.repl_tmpl, n));
+    CK(zeros(h, &q.repl_req, n * std::max(R, 1)));
+    CK(zeros(h, &q.repl_sflags, n * std::max(K, 1)));
+    CK(zeros(h, &q.repl_smask, n * std::max(K, 1)));
+    if (t.has_bounds) {
+      CK(zeros(h, &q.repl_sgte, n * std::max(K, 1)));
+      CK(zeros(h, &q.repl_slte, n * std::max(K, 1)));
+    }
+    if (in->export_price_order) {
+      CK(zeros(h, &q.repl_order, n * order_cap));
+      CK(zeros(h, &q.repl_order_n, n));
+    }
+    return KP_OK;
+  };
+  // `slots` x the per-slot count of each scratch array the pass needs (KP_CONSOL_SCRATCH, KP_SORT_SCRATCH)
+#define KP_ALLOC_SCRATCH(f, type, count, present) \
+  if (present) CK(zeros(h, &q.ws.f, slots * (size_t)(count)));
   for (int s = 0; s < S; s++)
     for (int i = in->subset_off[s]; i < in->subset_off[s + 1]; i++)
       if (in->subset_nodes[i] < 0 || in->subset_nodes[i] >= E) return h->err = "subset node out of range", KP_ERR_INVALID;
@@ -1638,26 +1648,10 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
       int32_t *d_soff, *d_snodes;
       CK(up_raw(h, &d_soff, soff.data(), soff.size()));
       CK(up_raw(h, &d_snodes, snodes_all.data(), std::max<size_t>(snodes_all.size(), 1)));
-      const size_t nb1 = (size_t)nb;
-      CK(zeros(h, &q.sort_key, nb1 * (size_t)std::max(T, 1)));
-      CK(zeros(h, &q.sort_val, nb1 * (size_t)std::max(T, 1)));
-      CK(zeros(h, &q.sort_bits, nb1 * (size_t)std::max(ITW, 1)));
-      CK(zeros(h, &q.decision, nb1));
-      CK(zeros(h, &q.replacement_its, nb1 * std::max(ITW, 1)));
-      CK(zeros(h, &q.n_new_claims, nb1));
-      CK(zeros(h, &q.n_unscheduled, nb1));
-      CK(zeros(h, &q.repl_tmpl, nb1));
-      CK(zeros(h, &q.repl_req, nb1 * std::max(R, 1)));
-      CK(zeros(h, &q.repl_sflags, nb1 * std::max(K, 1)));
-      CK(zeros(h, &q.repl_smask, nb1 * std::max(K, 1)));
-      if (t.has_bounds) {
-        CK(zeros(h, &q.repl_sgte, nb1 * std::max(K, 1)));
-        CK(zeros(h, &q.repl_slte, nb1 * std::max(K, 1)));
-      }
-      if (in->export_price_order) {
-        CK(zeros(h, &q.repl_order, nb1 * order_cap));
-        CK(zeros(h, &q.repl_order_n, nb1));
-      }
+      const size_t slots = (size_t)nb;  // k_decide_batch: block b uses sort slot b
+      KP_SORT_SCRATCH(KP_ALLOC_SCRATCH, d, q)
+      rc = alloc_rows(q, (size_t)nb);
+      if (rc != KP_OK) return rc;
       std::vector<int32_t> st;
       rc = run_solve(h, ms_left() < 0 ? 0 : std::max<int64_t>(ms_left(), 1), st);
       if (rc != KP_OK) return rc;
@@ -1689,8 +1683,7 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   for (int s = 0; s < S; s++) {
     int n = 0;
     for (int i = in->subset_off[s]; i < in->subset_off[s + 1]; i++) {
-      int node = in->subset_nodes[i];
-      if (node < 0 || node >= E) return h->err = "subset node out of range", KP_ERR_INVALID;
+      const int node = in->subset_nodes[i];
       n += in->node_pod_off[node + 1] - in->node_pod_off[node];
     }
     capq = std::max(capq, n);
@@ -1751,64 +1744,11 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_consolidate<false>, CONSOL_WARPS * 32, smem);
   per_sm = std::max(per_sm, 1);
   int grid = std::min(h->n_sm * per_sm, std::max(1, (S + CONSOL_WARPS - 1) / CONSOL_WARPS));
-  const size_t slots = (size_t)grid * CONSOL_WARPS, cq = (size_t)capq;
-  CK(zeros(h, &q.queue, slots * (cq + 1)));
-  CK(zeros(h, &q.qcls, slots * (cq + 1)));
-  CK(zeros(h, &q.last_len, slots * cq));
-  CK(zeros(h, &q.clsl, slots * cq));
-  CK(zeros(h, &q.rk, slots * cq));
-  if (n_extra > 0) CK(zeros(h, &q.kindl, slots * cq));
-  if (t.n_rsv > 0) {
-    CK(zeros(h, &q.rsv_cap, slots * (size_t)t.n_rsv));
-    CK(zeros(h, &q.c_rsv, slots * cq));
-  }
-  if (d.n_hostports > 0) {
-    CK(zeros(h, &q.c_ports, slots * cq));
-    CK(zeros(h, &q.ov_ports, slots * cq));
-  }
-  CK(zeros(h, &q.c_tmpl, slots * cq));
-  CK(zeros(h, &q.c_npods, slots * cq));
-  CK(zeros(h, &q.order, slots * cq));
-  CK(zeros(h, &q.cnt_at, slots * cq));
-  CK(zeros(h, &q.c_req, slots * cq * R));
-  CK(zeros(h, &q.c_sflags, slots * cq * K));
-  CK(zeros(h, &q.c_smask, slots * cq * K));
-  CK(zeros(h, &q.c_its, slots * cq * ITW));
-  CK(zeros(h, &q.c_j, slots * cq * R));
-  CK(zeros(h, &q.sort_key, slots * (size_t)std::max(T, 1)));
-  CK(zeros(h, &q.sort_val, slots * (size_t)std::max(T, 1)));
-  CK(zeros(h, &q.sort_bits, slots * (size_t)std::max(ITW, 1)));
-  CK(zeros(h, &q.cmask, slots * cq));
-  CK(zeros(h, &q.amask, slots * cq));
-  CK(zeros(h, &q.tmpl_remaining, slots * (size_t)std::max(N, 1) * R));
-  CK(zeros(h, &q.ov_node, slots * cq));
-  CK(zeros(h, &q.ov_rem, slots * cq * R));
-  CK(zeros(h, &q.ov_present, slots * cq));
-  CK(zeros(h, &q.ov_sflags, slots * cq * K));
-  CK(zeros(h, &q.ov_smask, slots * cq * K));
-  if (t.has_bounds) {
-    CK(zeros(h, &q.c_sgte, slots * cq * K));
-    CK(zeros(h, &q.c_slte, slots * cq * K));
-    CK(zeros(h, &q.ov_sgte, slots * cq * K));
-    CK(zeros(h, &q.ov_slte, slots * cq * K));
-  }
-  CK(zeros(h, &q.decision, (size_t)std::max(S, 1)));
-  CK(zeros(h, &q.replacement_its, (size_t)std::max(S, 1) * std::max(ITW, 1)));
-  CK(zeros(h, &q.n_new_claims, (size_t)std::max(S, 1)));
-  CK(zeros(h, &q.n_unscheduled, (size_t)std::max(S, 1)));
+  const size_t slots = (size_t)grid * CONSOL_WARPS;
+  KP_CONSOL_SCRATCH(KP_ALLOC_SCRATCH, d, q)
   const size_t S1 = (size_t)std::max(S, 1);
-  CK(zeros(h, &q.repl_tmpl, S1));
-  CK(zeros(h, &q.repl_req, S1 * std::max(R, 1)));
-  CK(zeros(h, &q.repl_sflags, S1 * std::max(K, 1)));
-  CK(zeros(h, &q.repl_smask, S1 * std::max(K, 1)));
-  if (t.has_bounds) {
-    CK(zeros(h, &q.repl_sgte, S1 * std::max(K, 1)));
-    CK(zeros(h, &q.repl_slte, S1 * std::max(K, 1)));
-  }
-  if (in->export_price_order) {
-    CK(zeros(h, &q.repl_order, S1 * order_cap));
-    CK(zeros(h, &q.repl_order_n, S1));
-  }
+  rc = alloc_rows(q, S1);
+  if (rc != KP_OK) return rc;
   CK(cudaMemsetAsync(q.decision, KP_DECISION_UNKNOWN, S1, h->stream));  // a subset the deadline cut off stays unknown
   CK(zeros(h, &q.next, 1));
   CK(zeros(h, &q.status, 1));
@@ -1864,3 +1804,4 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   }
   return KP_OK;
 }
+#undef KP_ALLOC_SCRATCH

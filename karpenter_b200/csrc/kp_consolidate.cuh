@@ -8,33 +8,48 @@
 //                   for every candidate subset: one warp per subset pulled from a global counter, 8 warps per CTA, all
 //                   SMs busy; the cluster's node table is shared read-only, each warp keeps the nodes its simulation
 //                   touched in a private overlay.
+//
+// Each memory layout a host sizes and a kernel carves is written out once, here: the staged read-only tables
+// (KP_STAGED_TABLES), the solver CTA's shared memory (SolveSmem) and k_consolidate's per-warp scratch
+// (KP_CONSOL_SCRATCH).
 #pragma once
 #include "kp_wsolve.cuh"
 
 #define KP_ALIGN16(x) (((x) + 15) & ~(size_t)15)
 
-// bytes of the state of the `ntk` groups on tk_key that a solver CTA keeps on chip (KpDev::tk_slot): the slot map, the
-// registered / populated masks and the counters with a stride of the key's value count (same formula on host and device)
-__host__ __device__ inline size_t kp_tk_bytes(const KpDev& d, int ntk) {
-  return KP_ALIGN16((size_t)d.G * 4) + 2 * KP_ALIGN16((size_t)ntk * 8) + KP_ALIGN16((size_t)ntk * d.tk_nv * 4);
-}
+// The read-only tables a kernel stages in shared memory, in order: field, element type, element count in the
+// dimensions of the KpDev `d`.  Each table starts 16-byte aligned.  kp_tab_bytes sizes them, stage_tables copies them.
+#define KP_STAGED_TABLES(X, d)                                    \
+  X(key_wellknown, uint8_t, d.K)                                  \
+  X(key_univ, uint64_t, d.K)                                      \
+  X(val_isint, uint64_t, d.K)                                     \
+  X(ge_off, int32_t, (size_t)d.R + 1)                             \
+  X(ge_vals, int64_t, d.n_ge)                                     \
+  X(ge_bits, uint64_t, (size_t)d.n_ge * d.ITW)                    \
+  X(itv_off, int32_t, (size_t)d.K + 1)                            \
+  X(itv, uint64_t, (size_t)d.n_itv * d.ITW)                       \
+  X(it_nokey, uint64_t, (size_t)d.K * d.ITW)                      \
+  X(it_dne, uint64_t, (size_t)d.K * d.ITW)                        \
+  X(it_nonempty, uint64_t, (size_t)d.K * d.ITW)                   \
+  X(it_valid, uint64_t, d.ITW)                                    \
+  X(off_slots, Slot, (size_t)(d.D > 0 ? d.D : 1) * d.K)           \
+  X(off_keys, uint32_t, d.D > 0 ? d.D : 1)                        \
+  X(offset_bits, uint64_t, (size_t)(d.D > 0 ? d.D : 1) * d.ITW)   \
+  X(tmpl_taintset, int32_t, d.N > 0 ? d.N : 1)                    \
+  X(nfit_sum, uint32_t, (size_t)d.n_rv * d.ESW)                   \
+  X(nstat_sum, uint32_t, (size_t)d.n_nsig * d.ESW)
 
-// bytes of the read-only tables staged in shared memory (same formula on host and device)
+// bytes of the staged tables
 __host__ __device__ inline size_t kp_tab_bytes(const KpDev& d) {
-  size_t K = d.K, R = d.R, ITW = d.ITW, D = d.D > 0 ? d.D : 1, N = d.N > 0 ? d.N : 1;
   size_t b = 0;
-  b += KP_ALIGN16(K) + 2 * KP_ALIGN16(8 * K);                    // key_wellknown, key_univ, val_isint
-  b += KP_ALIGN16(4 * (R + 1)) + KP_ALIGN16(8 * (size_t)d.n_ge) + KP_ALIGN16(8 * (size_t)d.n_ge * ITW);
-  b += KP_ALIGN16(4 * (K + 1)) + KP_ALIGN16(8 * (size_t)d.n_itv * ITW);
-  b += 3 * KP_ALIGN16(8 * K * ITW) + KP_ALIGN16(8 * ITW);        // it_nokey, it_dne, it_nonempty, it_valid
-  b += KP_ALIGN16(sizeof(Slot) * D * K) + KP_ALIGN16(4 * D) + KP_ALIGN16(8 * D * ITW);
-  b += KP_ALIGN16(4 * N);
-  b += KP_ALIGN16(4 * (size_t)d.n_rv * d.ESW) + KP_ALIGN16(4 * (size_t)d.n_nsig * d.ESW);  // candidate bitmap summaries
+#define KP_TAB_BYTES(field, type, count) b += KP_ALIGN16(sizeof(type) * (size_t)(count));
+  KP_STAGED_TABLES(KP_TAB_BYTES, d)
+#undef KP_TAB_BYTES
   return b;
 }
 
-// Copy the pointer block to shared memory and, when they fit, the small read-only tables next to it (key universe,
-// allocatable thresholds, bit-sliced instance-type rows, offering sets); patches the pointers. All threads of the CTA.
+// Copy the pointer block to shared memory and, when they fit, the staged tables next to it; patches the pointers.  All
+// threads of the CTA.
 __device__ __forceinline__ void stage_tables(const KpDev& d_in, KpDev* ds, unsigned char* tab) {
   const int tid = threadIdx.x, nt = blockDim.x;
   {
@@ -54,25 +69,7 @@ __device__ __forceinline__ void stage_tables(const KpDev& d_in, KpDev* ds, unsig
     if (tid == 0) ds->field = dst_;                                      \
     off += KP_ALIGN16(sizeof(type) * n_);                                \
   }
-    const size_t K_ = d_in.K, R_ = d_in.R, W_ = d_in.ITW, D_ = d_in.D > 0 ? d_in.D : 1, N_ = d_in.N > 0 ? d_in.N : 1;
-    KP_STAGE(key_wellknown, uint8_t, K_)
-    KP_STAGE(key_univ, uint64_t, K_)
-    KP_STAGE(val_isint, uint64_t, K_)
-    KP_STAGE(ge_off, int32_t, R_ + 1)
-    KP_STAGE(ge_vals, int64_t, d_in.n_ge)
-    KP_STAGE(ge_bits, uint64_t, (size_t)d_in.n_ge * W_)
-    KP_STAGE(itv_off, int32_t, K_ + 1)
-    KP_STAGE(itv, uint64_t, (size_t)d_in.n_itv * W_)
-    KP_STAGE(it_nokey, uint64_t, K_ * W_)
-    KP_STAGE(it_dne, uint64_t, K_ * W_)
-    KP_STAGE(it_nonempty, uint64_t, K_ * W_)
-    KP_STAGE(it_valid, uint64_t, W_)
-    KP_STAGE(off_slots, Slot, D_ * K_)
-    KP_STAGE(off_keys, uint32_t, D_)
-    KP_STAGE(offset_bits, uint64_t, D_ * W_)
-    KP_STAGE(tmpl_taintset, int32_t, N_)
-    KP_STAGE(nfit_sum, uint32_t, (size_t)d_in.n_rv * d_in.ESW)
-    KP_STAGE(nstat_sum, uint32_t, (size_t)d_in.n_nsig * d_in.ESW)
+    KP_STAGED_TABLES(KP_STAGE, d_in)
 #undef KP_STAGE
   }
   __syncthreads();
@@ -152,26 +149,61 @@ struct WSolveShared {
   Slot scratch[KP_MAXK];
 };
 
+// The solver CTA's dynamic shared memory: byte offset of every region and the total.  In order: the WSolveShared block;
+// the staged tables (tab_bytes); the state of the `ntk` groups on tk_key (slot map over all groups, registered /
+// populated masks, counters with a stride of tk_nv); the hot rows of the first CQ claims (requests, threshold rows); the
+// cold rows of the first CR (requirement masks, instance-type words, slot flags); the small arrays of the first CS
+// (failure masks, order, counts, template ids, c_dom).  An absent region takes no bytes.  plan_solve sizes the plan
+// with it, wsolve_cta carves its shared memory with it.
+struct SolveSmem {
+  size_t tab, tk_slot, tk_reg, tk_pop, tk_cnt, s_req, s_j, s_smask, s_its, s_sflags, cmask, amask, order, cnt_at, c_tmpl,
+      c_dom, total;
+  __host__ __device__ SolveSmem(const KpDev& d, size_t tab_bytes, int CS, int CQ, int CR, int ntk) {
+    size_t o = KP_ALIGN16(sizeof(WSolveShared));
+    auto at = [&o](size_t& r, size_t bytes) {
+      r = o;
+      o += bytes;
+    };
+    at(tab, tab_bytes);
+    const size_t tk = ntk > 0 ? ntk : 0, q = CQ > 0 ? CQ : 0, c = CR > 0 ? CR : 0, s = CS > 0 ? CS : 0;
+    at(tk_slot, tk ? KP_ALIGN16((size_t)d.G * 4) : 0);
+    at(tk_reg, KP_ALIGN16(tk * 8));
+    at(tk_pop, KP_ALIGN16(tk * 8));
+    at(tk_cnt, KP_ALIGN16(tk * d.tk_nv * 4));
+    at(s_req, KP_ALIGN16(q * d.R * 8));
+    at(s_j, KP_ALIGN16(q * d.R * 4));
+    at(s_smask, KP_ALIGN16(c * d.K * 8));
+    at(s_its, KP_ALIGN16(c * d.ITW * 8));
+    at(s_sflags, KP_ALIGN16(c * d.K));
+    at(cmask, s * 16);
+    at(amask, s * 8);
+    at(order, s * 4);
+    at(cnt_at, s * 4);
+    at(c_tmpl, s * 4);
+    at(c_dom, s);
+    total = o + 64;
+  }
+};
+
 // warp 0: the solver; warp 1: the pod stager (see StageRing)
 template <bool LEAN, bool COHORT, bool VOL>
 __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CQ, int CR, int ntk) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   WSolveShared& sh = *reinterpret_cast<WSolveShared*>(smem_raw);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  unsigned char* tab = smem_raw + KP_ALIGN16(sizeof(WSolveShared));
-  stage_tables(d_in, &sh.ds, tab);
+  stage_tables(d_in, &sh.ds, smem_raw + SolveSmem(d_in, 0, 0, 0, 0, 0).tab);
   const KpDev& d = sh.ds;
   WInst& I = sh.inst;
-  unsigned char* p = tab + d_in.tab_bytes;
+  const SolveSmem L(d, d.tab_bytes, CS, CQ, CR, ntk);
   int32_t* s_slot = nullptr;
   uint64_t *s_reg = nullptr, *s_pop = nullptr;
   int32_t* s_cnt = nullptr;
   if (ntk > 0) {  // the state of the groups on the topology key, numbered in group order (warp 0)
     const int nv = d_in.tk_nv;
-    s_slot = reinterpret_cast<int32_t*>(p);
-    s_reg = reinterpret_cast<uint64_t*>(p + KP_ALIGN16((size_t)d_in.G * 4));
-    s_pop = s_reg + KP_ALIGN16((size_t)ntk * 8) / 8;
-    s_cnt = reinterpret_cast<int32_t*>(s_pop + KP_ALIGN16((size_t)ntk * 8) / 8);
+    s_slot = reinterpret_cast<int32_t*>(smem_raw + L.tk_slot);
+    s_reg = reinterpret_cast<uint64_t*>(smem_raw + L.tk_reg);
+    s_pop = reinterpret_cast<uint64_t*>(smem_raw + L.tk_pop);
+    s_cnt = reinterpret_cast<int32_t*>(smem_raw + L.tk_cnt);
     if (warp == 0) {
       for (int base = 0, n = 0; base < d_in.G; base += 32) {
         const int g = base + lane;
@@ -188,7 +220,6 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CQ, in
         n += __popc(m);
       }
     }
-    p += kp_tk_bytes(d_in, ntk);
   }
   const int Cmax = d.Cmax;
   if (threadIdx.x == 0) {
@@ -256,34 +287,24 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CQ, in
       sh.ds.tk_pop = s_pop;
       sh.ds.tk_cnt = s_cnt;
     }
-    if (CQ > 0) {  // hot rows of the first CQ claims (same formula as kp_api.cu plan_solve)
-      I.s_req = reinterpret_cast<int64_t*>(p);
-      p += KP_ALIGN16((size_t)CQ * d.R * 8);
-      I.s_j = reinterpret_cast<int32_t*>(p);
-      p += KP_ALIGN16((size_t)CQ * d.R * 4);
+    if (CQ > 0) {  // hot rows of the first CQ claims
+      I.s_req = reinterpret_cast<int64_t*>(smem_raw + L.s_req);
+      I.s_j = reinterpret_cast<int32_t*>(smem_raw + L.s_j);
       I.CQ = CQ;
     }
     if (CR > 0) {  // cold rows of the first CR claims
-      I.s_smask = reinterpret_cast<uint64_t*>(p);
-      p += KP_ALIGN16((size_t)CR * d.K * 8);
-      I.s_its = reinterpret_cast<uint64_t*>(p);
-      p += KP_ALIGN16((size_t)CR * d.ITW * 8);
-      I.s_sflags = reinterpret_cast<uint8_t*>(p);
-      p += KP_ALIGN16((size_t)CR * d.K);
+      I.s_smask = reinterpret_cast<uint64_t*>(smem_raw + L.s_smask);
+      I.s_its = reinterpret_cast<uint64_t*>(smem_raw + L.s_its);
+      I.s_sflags = reinterpret_cast<uint8_t*>(smem_raw + L.s_sflags);
       I.CR = CR;
     }
     if (CS > 0) {  // claim order, template ids and the failure masks of the first CS claims live in shared memory
-      I.cmask = reinterpret_cast<ulonglong2*>(p);
-      p += (size_t)CS * 16;
-      I.amask = reinterpret_cast<unsigned long long*>(p);
-      p += (size_t)CS * 8;
-      I.order = reinterpret_cast<int32_t*>(p);
-      p += (size_t)CS * 4;
-      I.cnt_at = reinterpret_cast<int32_t*>(p);
-      p += (size_t)CS * 4;
-      I.c_tmpl = reinterpret_cast<int32_t*>(p);
-      p += (size_t)CS * 4;
-      I.c_dom = reinterpret_cast<uint8_t*>(p);
+      I.cmask = reinterpret_cast<ulonglong2*>(smem_raw + L.cmask);
+      I.amask = reinterpret_cast<unsigned long long*>(smem_raw + L.amask);
+      I.order = reinterpret_cast<int32_t*>(smem_raw + L.order);
+      I.cnt_at = reinterpret_cast<int32_t*>(smem_raw + L.cnt_at);
+      I.c_tmpl = reinterpret_cast<int32_t*>(smem_raw + L.c_tmpl);
+      I.c_dom = reinterpret_cast<uint8_t*>(smem_raw + L.c_dom);
       I.CS = CS;
     }
   }
@@ -346,6 +367,55 @@ __global__ void __launch_bounds__(64, 1) k_wsolve_batch(const KpDev* __restrict_
 
 // ---------------------------------------------------------------------------------------------------------------
 // Consolidation.
+
+// k_consolidate's per-warp scratch, in allocation order: field, element type, elements per warp slot in the dimensions
+// of the KpDev `d` and the KpConsol `q`, whether the pass needs it.  The host allocates slots x count of each field it
+// needs (one array per field); consol_slot points warp `slot` at elements [slot * count, (slot + 1) * count) of each,
+// null where the pass lacks the field.  KP_SORT_SCRATCH is what consol_decide uses: the instance types of the single new
+// NodeClaim in price order (sort keys / ids) and a bitmap; the general path allocates it alone, one slot per instance.
+#define KP_SORT_SCRATCH(X, d, q)                                     \
+  X(sort_key, double, q.T, true)                                     \
+  X(sort_val, int32_t, q.T, true)                                    \
+  X(sort_bits, unsigned long long, d.ITW, true)
+#define KP_CONSOL_SCRATCH(X, d, q)                                   \
+  X(queue, int32_t, (size_t)q.capq + 1, true)                        \
+  X(qcls, int32_t, (size_t)q.capq + 1, true)                         \
+  X(last_len, int32_t, q.capq, true)                                 \
+  X(clsl, int32_t, q.capq, true)                                     \
+  X(rk, int32_t, q.capq, true)                                       \
+  X(kindl, uint8_t, q.capq, q.n_extra > 0) /* kind of local pod i, 0: candidate pod */ \
+  X(rsv_cap, int32_t, d.n_rsv, d.n_rsv > 0) /* the simulation's own ReservationManager */ \
+  X(c_rsv, unsigned long long, q.capq, d.n_rsv > 0)                  \
+  X(c_ports, unsigned long long, q.capq, d.n_hostports > 0) /* host ports of the claims / touched nodes */ \
+  X(ov_ports, unsigned long long, q.capq, d.n_hostports > 0)         \
+  X(c_tmpl, int32_t, q.capq, true)                                   \
+  X(c_npods, int32_t, q.capq, true)                                  \
+  X(order, int32_t, q.capq, true)                                    \
+  X(cnt_at, int32_t, q.capq, true)                                   \
+  X(c_req, int64_t, (size_t)q.capq * d.R, true)                      \
+  X(c_sflags, uint8_t, (size_t)q.capq * d.K, true)                   \
+  X(c_smask, uint64_t, (size_t)q.capq * d.K, true)                   \
+  X(c_its, uint64_t, (size_t)q.capq * d.ITW, true)                   \
+  X(c_j, int32_t, (size_t)q.capq * d.R, true)                        \
+  KP_SORT_SCRATCH(X, d, q)                                           \
+  X(cmask, ulonglong2, q.capq, true)                                 \
+  X(amask, unsigned long long, q.capq, true)                         \
+  X(tmpl_remaining, int64_t, (size_t)(d.N > 0 ? d.N : 1) * d.R, true) \
+  X(ov_node, int32_t, q.capq, true)                                  \
+  X(ov_rem, int64_t, (size_t)q.capq * d.R, true)                     \
+  X(ov_present, uint32_t, q.capq, true)                              \
+  X(ov_sflags, uint8_t, (size_t)q.capq * d.K, true)                  \
+  X(ov_smask, uint64_t, (size_t)q.capq * d.K, true)                  \
+  X(c_sgte, int64_t, (size_t)q.capq * d.K, d.has_bounds)             \
+  X(c_slte, int64_t, (size_t)q.capq * d.K, d.has_bounds)             \
+  X(ov_sgte, int64_t, (size_t)q.capq * d.K, d.has_bounds)            \
+  X(ov_slte, int64_t, (size_t)q.capq * d.K, d.has_bounds)
+struct ConsolScratch {
+#define KP_SCRATCH_FIELD(f, type, count, present) type* f;
+  KP_CONSOL_SCRATCH(KP_SCRATCH_FIELD, , )
+#undef KP_SCRATCH_FIELD
+};
+
 struct KpConsol {
   // inputs
   int n_subsets;
@@ -373,41 +443,16 @@ struct KpConsol {
   const int32_t* ml_set;
   const double* ml_price;
   int T;
-  // per warp slot: instance types of the single new NodeClaim in price order (sort keys / ids), bitmap scratch
-  double* sort_key;              // [slots * T]
-  int32_t* sort_val;             // [slots * T]
-  unsigned long long* sort_bits; // [slots * ITW]
   int ct_key, ct_spot, ct_od, ct_order_valid;  // bit i of ct_order_valid: ct_order[i] is interned
   int spot_to_spot_enabled;
   // pods every simulation schedules besides the candidates' (helpers.go:65-91): rows extra_row0 .. extra_row0+n_extra-1
   int n_extra, extra_row0;
   const uint8_t* extra_kind;     // [n_extra] KP_EXTRA_*
-  uint8_t* kindl;                // per warp slot [capq]: kind of local pod i (0: candidate pod)
-  int32_t* rsv_cap;              // per warp slot [n_rsv]: the simulation's own ReservationManager
-  unsigned long long* c_rsv;     // per warp slot [capq]
-  unsigned long long *c_ports, *ov_ports;  // per warp slot [capq]: host ports of the simulation's claims / touched nodes
   // context deadline: the first warp to start stamps t_start; a warp that finds deadline_ns used up stops pulling work
   long long deadline_ns;
   unsigned long long* t_start;
-  // per warp slot scratch
   int capq;                      // pods / claims / overlay entries an instance can hold
-  int32_t *queue, *qcls, *last_len, *clsl, *rk;
-  int32_t *c_tmpl, *c_npods, *order, *cnt_at;
-  int64_t* c_req;
-  uint8_t* c_sflags;
-  uint64_t* c_smask;
-  int64_t *c_sgte, *c_slte;
-  uint64_t* c_its;
-  int32_t* c_j;
-  ulonglong2* cmask;
-  unsigned long long* amask;
-  int64_t* tmpl_remaining;
-  int32_t* ov_node;
-  int64_t* ov_rem;
-  uint32_t* ov_present;
-  uint8_t* ov_sflags;
-  uint64_t* ov_smask;
-  int64_t *ov_sgte, *ov_slte;
+  ConsolScratch ws;              // per warp slot scratch (KP_CONSOL_SCRATCH): the arrays of all slots
   // outputs
   uint8_t* decision;             // [n_subsets] KP_DECISION_*, 255 = needs a feature that is not built
   uint64_t* replacement_its;     // [n_subsets * ITW]
@@ -426,6 +471,15 @@ struct KpConsol {
   int32_t* next;                 // work counter
   int32_t* status;
 };
+
+// warp slot `slot`'s share of the per-warp scratch
+__device__ __forceinline__ ConsolScratch consol_slot(const KpDev& d, const KpConsol& q, size_t slot) {
+  ConsolScratch w;
+#define KP_SCRATCH_SLOT(f, type, count, present) w.f = (present) ? q.ws.f + slot * (size_t)(count) : nullptr;
+  KP_CONSOL_SCRATCH(KP_SCRATCH_SLOT, d, q)
+#undef KP_SCRATCH_SLOT
+  return w;
+}
 
 // computeConsolidation (consolidation.go:136-229) for one simulated candidate set: `unscheduled` pods could not be
 // placed (or only on uninitialized nodes), `n_new` NodeClaims were opened; claim 0's row (requirement slots, instance
@@ -521,9 +575,10 @@ __device__ __forceinline__ void consol_decide(const KpDev& d, const KpConsol& q,
       uint64_t cur = its;  // lane w: word w of the NodeClaim's instance types as they go through the steps below
       // ---- OrderByPrice + Truncate(600) (helpers.go:120, scheduler.go:361-379, types.go:238-257,339-351).  The order
       // only matters when it truncates, or for the 15-cheapest rule of single-node spot-to-spot consolidation.
-      double* sk = q.sort_key + slot * (size_t)q.T;
-      int32_t* sv = q.sort_val + slot * (size_t)q.T;
-      unsigned long long* sb = q.sort_bits + slot * (size_t)ITW;
+      const ConsolScratch w = consol_slot(d, q, slot);
+      double* sk = w.sort_key;
+      int32_t* sv = w.sort_val;
+      unsigned long long* sb = w.sort_bits;
       int n_ord = 0;
       const bool need_order = n_its > 600 || (spot_path && q.spot_to_spot_enabled) || q.export_order;
       if (need_order) {
@@ -752,30 +807,31 @@ __global__ void __launch_bounds__(CONSOL_WARPS * 32, CONSOL_MIN_CTAS) k_consolid
   const KpDev& d = sh.ds;
   ConsolWarp& W = sh.w[warp];
   WInst& I = W.inst;
-  const int K = d.K, R = d.R, ITW = d.ITW, N = d.N;
+  const int R = d.R, N = d.N;
   const size_t slot = (size_t)blockIdx.x * CONSOL_WARPS + warp;
   const int capq = q.capq;
+  const ConsolScratch w = consol_slot(d, q, slot);
   if (lane == 0) {
-    I.queue = q.queue + slot * (capq + 1);
-    I.qcls = q.qcls + slot * (capq + 1);
-    I.last_len = q.last_len + slot * capq;
+    I.queue = w.queue;
+    I.qcls = w.qcls;
+    I.last_len = w.last_len;
     I.pod_target = nullptr;
     I.pod_error = nullptr;
     I.Cmax = capq;
-    I.c_tmpl = q.c_tmpl + slot * capq;
-    I.c_npods = q.c_npods + slot * capq;
-    I.c_req = q.c_req + slot * capq * R;
-    I.c_sflags = q.c_sflags + slot * capq * K;
-    I.c_smask = q.c_smask + slot * capq * K;
-    I.c_sgte = q.c_sgte ? q.c_sgte + slot * capq * K : nullptr;
-    I.c_slte = q.c_slte ? q.c_slte + slot * capq * K : nullptr;
-    I.c_its = q.c_its + slot * capq * ITW;
-    I.c_j = q.c_j + slot * capq * R;
-    I.order = q.order + slot * capq;
-    I.cnt_at = q.cnt_at + slot * capq;
-    I.cmask = q.cmask + slot * capq;
-    I.amask = q.amask + slot * capq;
-    I.tmpl_remaining = q.tmpl_remaining + slot * (size_t)(N > 0 ? N : 1) * R;
+    I.c_tmpl = w.c_tmpl;
+    I.c_npods = w.c_npods;
+    I.c_req = w.c_req;
+    I.c_sflags = w.c_sflags;
+    I.c_smask = w.c_smask;
+    I.c_sgte = w.c_sgte;
+    I.c_slte = w.c_slte;
+    I.c_its = w.c_its;
+    I.c_j = w.c_j;
+    I.order = w.order;
+    I.cnt_at = w.cnt_at;
+    I.cmask = w.cmask;
+    I.amask = w.amask;
+    I.tmpl_remaining = w.tmpl_remaining;
     I.node_rem = d.node_rem;  // shared base, read-only here
     I.node_rem_present = d.node_rem_present;
     I.node_sflags = d.node_sflags;
@@ -793,24 +849,24 @@ __global__ void __launch_bounds__(CONSOL_WARPS * 32, CONSOL_MIN_CTAS) k_consolid
     I.CR = 0;
     I.c_dom = nullptr;  // candidate sets with topology take the batch path (k_wsolve_batch)
     I.g_c_dom = nullptr;
-    I.rsv_cap = d.n_rsv ? q.rsv_cap + slot * d.n_rsv : nullptr;
-    I.c_rsv = d.n_rsv ? q.c_rsv + slot * capq : nullptr;
-    I.c_ports = d.n_hostports ? q.c_ports + slot * capq : nullptr;
-    I.ov_ports = d.n_hostports ? q.ov_ports + slot * capq : nullptr;
+    I.rsv_cap = w.rsv_cap;
+    I.c_rsv = w.c_rsv;
+    I.c_ports = w.c_ports;
+    I.ov_ports = w.ov_ports;
     I.node_ports = d.node_ports;  // shared base, read-only here
     I.ov_cap = capq;
-    I.ov_node = q.ov_node + slot * capq;
-    I.ov_rem = q.ov_rem + slot * capq * R;
-    I.ov_present = q.ov_present + slot * capq;
-    I.ov_sflags = q.ov_sflags + slot * capq * K;
-    I.ov_smask = q.ov_smask + slot * capq * K;
-    I.ov_sgte = q.ov_sgte ? q.ov_sgte + slot * capq * K : nullptr;
-    I.ov_slte = q.ov_slte ? q.ov_slte + slot * capq * K : nullptr;
+    I.ov_node = w.ov_node;
+    I.ov_rem = w.ov_rem;
+    I.ov_present = w.ov_present;
+    I.ov_sflags = w.ov_sflags;
+    I.ov_smask = w.ov_smask;
+    I.ov_sgte = w.ov_sgte;
+    I.ov_slte = w.ov_slte;
   }
   __syncwarp();
-  int32_t* clsl = q.clsl + slot * capq;
-  int32_t* rk = q.rk + slot * capq;
-  uint8_t* kindl = q.n_extra > 0 ? q.kindl + slot * capq : nullptr;
+  int32_t* clsl = w.clsl;
+  int32_t* rk = w.rk;
+  uint8_t* kindl = w.kindl;
   if (lane == 0) I.pod_kind = kindl;
   unsigned long long t0 = 0;
   if (q.deadline_ns > 0) {

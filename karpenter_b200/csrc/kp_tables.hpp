@@ -174,7 +174,6 @@ struct KpDev {
   int32_t* node_npods;            // [E]
   // claims (dynamic)
   int Cmax;
-  int CS;                         // claim positions / ids mirrored in shared memory
   int32_t* c_tmpl;                // [Cmax]
   int32_t* c_npods;
   int64_t* c_req;                 // [Cmax*R]
