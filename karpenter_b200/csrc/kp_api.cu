@@ -688,8 +688,6 @@ static void plan_solve(Instance& in) {
     CR = 0;
     while (CR + 32 <= CQ && layout(0, CQ, CR + 32).cmask - whole.s_req <= rows) CR += 32;
   }
-  if (getenv("KP_CS_LIMIT")) CQ = std::min(CQ, 32);
-  CR = std::min(CR, CQ);
   // ... and claim order / failure masks of the first CS claims
   int CS = 0;
   if (layout(64, CQ, CR).total <= budget) {  // the largest multiple of 32 that fits, capped at Cmax
@@ -704,7 +702,25 @@ static void plan_solve(Instance& in) {
     }
     CS = lo;
   }
-  if (const char* lim = getenv("KP_CS_LIMIT")) CS = std::min(CS, std::max(0, atoi(lim)) / 32 * 32);  // test knob
+  // KP_SMEM_CAP="CS,CQ,CR,TK" (test knob): upper bounds on the plan, an empty field leaves that part as planned.  They only
+  // lower it, so every capped layout is one the kernel is already handed: CS stays a multiple of 32, CR <= CQ, and a TK
+  // below the number of groups on the topology key leaves their state in global memory.
+  if (const char* cap = getenv("KP_SMEM_CAP")) {
+    long v[4];
+    bool set[4] = {false, false, false, false};
+    for (int f = 0; f < 4 && cap; f++) {
+      char* end;
+      v[f] = std::max(0l, strtol(cap, &end, 10));
+      set[f] = end != cap;
+      cap = strchr(cap, ',');
+      if (cap) cap++;
+    }
+    if (set[0]) CS = (int)std::min<long>(CS, v[0] / 32 * 32);
+    if (set[1]) CQ = (int)std::min<long>(CQ, v[1]);
+    if (set[2]) CR = (int)std::min<long>(CR, v[2]);
+    if (set[3] && v[3] < in.tk_groups) in.tk_groups = 0;
+  }
+  CR = std::min(CR, CQ);
   in.lean = in.host.G == 0 && !in.host.has_bounds && !in.host.min_values_strict && in.host.n_rsv == 0 && d.n_hostports == 0 &&
             !in.host.has_vol_alts && !getenv("KP_NO_LEAN");
   if (in.host.has_vol_alts) in.cohort = false;  // (the volume-alternative instantiation exists without cohorts only)

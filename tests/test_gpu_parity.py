@@ -283,9 +283,10 @@ def test_library_counter_table_single_gpu(handle):
 
 
 def test_shared_to_global_migration(monkeypatch):
-    """Claims outgrow the shared-memory copies of the claim order / failure bitmaps (forced early with KP_CS_LIMIT):
-    the solver migrates them to HBM mid-run and the result must not change."""
-    monkeypatch.setenv("KP_CS_LIMIT", "64")
+    """Claims outgrow the shared-memory copies of the claim order / failure bitmaps (forced early with KP_SMEM_CAP: at
+    most 64 claims' small arrays and 32 claims' rows on chip): the solver migrates them to HBM mid-run and the result
+    must not change."""
+    monkeypatch.setenv("KP_SMEM_CAP", "64,32,,")
     h = _native.Handle()
     try:
         for enc, what in ((workloads.config_c2(n_pods=30000, n_its=500), "C2 migrate "),
