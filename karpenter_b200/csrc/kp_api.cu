@@ -547,7 +547,7 @@ static int upload_tables(kp_handle* h, Instance& in, const kp_problem* p, int cm
   CK(zeros(h, &d.c_j, C * t.R));
   CK(zeros(h, &d.order, C));
   CK(zeros(h, &d.cnt_at, C));
-  CK(zeros(h, &d.cmask, C));
+  CK(zeros(h, &d.pmask, C));
   CK(zeros(h, &d.amask, C));
   CK(zeros(h, &d.c_dom, C));
   // host ports
@@ -627,7 +627,7 @@ static int reset_dynamic(kp_handle* h, Instance& in) {
   CK(cudaMemsetAsync(d.node_npods, 0, (size_t)std::max(t.E, 1) * 4, h->stream));
   size_t C = (size_t)d.Cmax;
   CK(cudaMemsetAsync(d.c_npods, 0, C * 4, h->stream));
-  CK(cudaMemsetAsync(d.cmask, 0, C * sizeof(ulonglong2), h->stream));
+  CK(cudaMemsetAsync(d.pmask, 0, C * sizeof(ulonglong2), h->stream));
   CK(cudaMemsetAsync(d.amask, 0, C * 8, h->stream));
   CK(cudaMemsetAsync(d.c_rsv, 0, C * 8, h->stream));
   if (in.d_dropped) CK(cudaMemsetAsync(in.d_dropped, 0, C, h->stream));
@@ -674,19 +674,19 @@ static void plan_solve(Instance& in) {
   // claim rows: hot = requests + threshold row, cold = requirement slots + instance-type words.  The rows get what whole
   // rows of up to 512 claims take within half the budget; the small arrays keep the rest.
   int CR = std::min(d.Cmax, 512);
-  while (CR > 0 && layout(0, CR, CR).cmask > budget / 2) CR -= 32;
+  while (CR > 0 && layout(0, CR, CR).pmask > budget / 2) CR -= 32;
   CR = std::max(CR, 0);
   const SolveSmem whole = layout(0, CR, CR);
-  const size_t rows = whole.cmask - whole.s_req;
+  const size_t rows = whole.pmask - whole.s_req;
   int CQ = CR;
   // With classes on the domain fast path almost every commit is fp_fit + a store of the hot row: claims are visited
   // round-robin, so the hot rows of as many claims as possible (C3: all of them) beat whole rows of a few hundred.
   // Cold rows take what is left.
   if (dom_fp) {
     CQ = std::min((d.Cmax + 31) / 32 * 32, (int)(rows / ((size_t)d.R * 12 + 1)) / 32 * 32);
-    while (CQ > 0 && layout(0, CQ, 0).cmask - whole.s_req > rows) CQ -= 32;
+    while (CQ > 0 && layout(0, CQ, 0).pmask - whole.s_req > rows) CQ -= 32;
     CR = 0;
-    while (CR + 32 <= CQ && layout(0, CQ, CR + 32).cmask - whole.s_req <= rows) CR += 32;
+    while (CR + 32 <= CQ && layout(0, CQ, CR + 32).pmask - whole.s_req <= rows) CR += 32;
   }
   // ... and claim order / failure masks of the first CS claims
   int CS = 0;
@@ -1294,13 +1294,14 @@ double kp_comm_last_allreduce_ms(kp_handle* h) { return h->allreduce_ms; }
 
 #ifdef KP_PHASE_PROF
 // Profiling build only: the solver warp's cycles per phase of the last solve of an instance (see KP_PROF_LAP), out[p] for
-// p < KP_NPHASE, then the cycles of the whole pod loop.  Returns the number of values written.
+// p < KP_NPHASE, then the cycles of the whole pod loop, then the in-flight scan's steps, the positions it walked up to
+// its results and the cycles of its first 32-wide steps.  Returns the number of values written.
 int kp_phase_profile(kp_handle* h, int32_t instance, int64_t* out, int32_t n) {
   Instance* in = pick_instance(h, instance);
-  if (!in || n < KP_NPHASE + 1) return h->err = "kp_phase_profile: no such instance or buffer too small", -1;
+  if (!in || n < KP_NPROF) return h->err = "kp_phase_profile: no such instance or buffer too small", -1;
   cudaSetDevice(h->device);
-  CK(cudaMemcpy(out, in->dev.counters + KP_PROF_AT, (KP_NPHASE + 1) * 8, cudaMemcpyDeviceToHost));
-  return KP_NPHASE + 1;
+  CK(cudaMemcpy(out, in->dev.counters + KP_PROF_AT, KP_NPROF * 8, cudaMemcpyDeviceToHost));
+  return KP_NPROF;
 }
 #endif
 

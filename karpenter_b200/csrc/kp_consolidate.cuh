@@ -156,7 +156,7 @@ struct WSolveShared {
 // (failure masks, order, counts, template ids, c_dom).  An absent region takes no bytes.  plan_solve sizes the plan
 // with it, wsolve_cta carves its shared memory with it.
 struct SolveSmem {
-  size_t tab, tk_slot, tk_reg, tk_pop, tk_cnt, s_req, s_j, s_smask, s_its, s_sflags, cmask, amask, order, cnt_at, c_tmpl,
+  size_t tab, tk_slot, tk_reg, tk_pop, tk_cnt, s_req, s_j, s_smask, s_its, s_sflags, pmask, amask, order, cnt_at, c_tmpl,
       c_dom, total;
   __host__ __device__ SolveSmem(const KpDev& d, size_t tab_bytes, int CS, int CQ, int CR, int ntk) {
     size_t o = KP_ALIGN16(sizeof(WSolveShared));
@@ -175,7 +175,7 @@ struct SolveSmem {
     at(s_smask, KP_ALIGN16(c * d.K * 8));
     at(s_its, KP_ALIGN16(c * d.ITW * 8));
     at(s_sflags, KP_ALIGN16(c * d.K));
-    at(cmask, s * 16);
+    at(pmask, s * 16);
     at(amask, s * 8);
     at(order, s * 4);
     at(cnt_at, s * 4);
@@ -247,7 +247,7 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CQ, in
     I.c_j = d.c_j;
     I.order = d.order;
     I.cnt_at = d.cnt_at;
-    I.cmask = d.cmask;
+    I.pmask = d.pmask;
     I.amask = d.amask;
     I.tmpl_remaining = d.tmpl_remaining;
     I.node_rem = d.node_rem;
@@ -270,7 +270,7 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CQ, in
     I.g_order = d.order;
     I.g_cnt_at = d.cnt_at;
     I.g_c_tmpl = d.c_tmpl;
-    I.g_cmask = d.cmask;
+    I.g_pmask = d.pmask;
     I.g_amask = d.amask;
     I.c_dom = d.c_dom;
     I.g_c_dom = d.c_dom;
@@ -299,7 +299,7 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CQ, in
       I.CR = CR;
     }
     if (CS > 0) {  // claim order, template ids and the failure masks of the first CS claims live in shared memory
-      I.cmask = reinterpret_cast<ulonglong2*>(smem_raw + L.cmask);
+      I.pmask = reinterpret_cast<ulonglong2*>(smem_raw + L.pmask);
       I.amask = reinterpret_cast<unsigned long long*>(smem_raw + L.amask);
       I.order = reinterpret_cast<int32_t*>(smem_raw + L.order);
       I.cnt_at = reinterpret_cast<int32_t*>(smem_raw + L.cnt_at);
@@ -350,6 +350,9 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CQ, in
 #ifdef KP_PHASE_PROF
     for (int p = 0; p < KP_NPHASE; p++) d.counters[KP_PROF_AT + p] = I.prof[p];
     d.counters[KP_PROF_AT + KP_NPHASE] = I.prof_total;
+    d.counters[KP_PROF_AT + KP_NPHASE + 1] = I.scan_steps;
+    d.counters[KP_PROF_AT + KP_NPHASE + 2] = I.scan_pos;
+    d.counters[KP_PROF_AT + KP_NPHASE + 3] = I.scan_first_cyc;
 #endif
   }
 }
@@ -398,7 +401,7 @@ __global__ void __launch_bounds__(64, 1) k_wsolve_batch(const KpDev* __restrict_
   X(c_its, uint64_t, (size_t)q.capq * d.ITW, true)                   \
   X(c_j, int32_t, (size_t)q.capq * d.R, true)                        \
   KP_SORT_SCRATCH(X, d, q)                                           \
-  X(cmask, ulonglong2, q.capq, true)                                 \
+  X(pmask, ulonglong2, q.capq, true)                                 \
   X(amask, unsigned long long, q.capq, true)                         \
   X(tmpl_remaining, int64_t, (size_t)(d.N > 0 ? d.N : 1) * d.R, true) \
   X(ov_node, int32_t, q.capq, true)                                  \
@@ -829,7 +832,7 @@ __global__ void __launch_bounds__(CONSOL_WARPS * 32, CONSOL_MIN_CTAS) k_consolid
     I.c_j = w.c_j;
     I.order = w.order;
     I.cnt_at = w.cnt_at;
-    I.cmask = w.cmask;
+    I.pmask = w.pmask;
     I.amask = w.amask;
     I.tmpl_remaining = w.tmpl_remaining;
     I.node_rem = d.node_rem;  // shared base, read-only here

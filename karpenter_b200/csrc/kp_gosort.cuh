@@ -13,11 +13,13 @@
 #define FULL 0xffffffffu
 #endif
 
-template <class K>
+// PM: a second payload by position, moved with `val` (the claim order's failure masks)
+template <class K, bool PM = false>
 struct WarpSorterT {
   K* key;    // sort key by position (pod count of a claim; price of an instance type)
   int* val;  // payload by position
   int lane;
+  ulonglong2* pm;
 
   __device__ bool less(int i, int j) const { return key[i] < key[j]; }
   __device__ void swap(int i, int j) {
@@ -28,6 +30,11 @@ struct WarpSorterT {
       int t = val[i];
       val[i] = val[j];
       val[j] = t;
+      if (PM) {
+        const ulonglong2 tp = pm[i];
+        pm[i] = pm[j];
+        pm[j] = tp;
+      }
     }
     __syncwarp();
   }
@@ -71,24 +78,30 @@ struct WarpSorterT {
   __device__ void rotate_right(int to, int from) {
     const K ek = key[from];
     const int ev = val[from];
+    ulonglong2 ep = {};
+    if (PM) ep = pm[from];
     for (int b0 = from; b0 > to; b0 -= 32) {
       const int i = b0 - lane;
       K vk = 0;
       int vv = 0;
+      ulonglong2 vp = {};
       if (i > to) {
         vk = key[i - 1];
         vv = val[i - 1];
+        if (PM) vp = pm[i - 1];
       }
       __syncwarp();
       if (i > to) {
         key[i] = vk;
         val[i] = vv;
+        if (PM) pm[i] = vp;
       }
       __syncwarp();
     }
     if (lane == 0) {
       key[to] = ek;
       val[to] = ev;
+      if (PM) pm[to] = ep;
     }
     __syncwarp();
   }
@@ -96,24 +109,30 @@ struct WarpSorterT {
   __device__ void rotate_left(int from, int to) {
     const K ek = key[from];
     const int ev = val[from];
+    ulonglong2 ep = {};
+    if (PM) ep = pm[from];
     for (int b0 = from; b0 < to; b0 += 32) {
       const int i = b0 + lane;
       K vk = 0;
       int vv = 0;
+      ulonglong2 vp = {};
       if (i < to) {
         vk = key[i + 1];
         vv = val[i + 1];
+        if (PM) vp = pm[i + 1];
       }
       __syncwarp();
       if (i < to) {
         key[i] = vk;
         val[i] = vv;
+        if (PM) pm[i] = vp;
       }
       __syncwarp();
     }
     if (lane == 0) {
       key[to] = ek;
       val[to] = ev;
+      if (PM) pm[to] = ep;
     }
     __syncwarp();
   }
@@ -122,9 +141,11 @@ struct WarpSorterT {
     const int n = b - a;
     K k = 0;
     int v = 0;
+    ulonglong2 p = {};
     if (lane < n) {
       k = key[a + lane];
       v = val[a + lane];
+      if (PM) p = pm[a + lane];
     }
     int rank = 0;
     for (int j = 0; j < n; j++) {
@@ -135,6 +156,7 @@ struct WarpSorterT {
     if (lane < n) {
       key[a + rank] = k;
       val[a + rank] = v;
+      if (PM) pm[a + rank] = p;
     }
     __syncwarp();
   }
@@ -303,6 +325,11 @@ struct WarpSorterT {
         val[i] = val[j];
         key[j] = tk;
         val[j] = tv;
+        if (PM) {
+          const ulonglong2 tp = pm[i];
+          pm[i] = pm[j];
+          pm[j] = tp;
+        }
       }
     }
     __syncwarp();

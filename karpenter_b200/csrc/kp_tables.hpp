@@ -188,8 +188,8 @@ struct KpDev {
   // monotone failure cache: for a topology-free class whose keys can never be "undefined" on a NodeClaim, CanAdd only
   // ever flips from true to false (requirements tighten, requests grow, instance types shrink: nodeclaim.go:207-219)
   int n_fsig;                     // distinct requirement sets of such classes
-  ulonglong2* cmask;              // [Cmax] per claim: x = rejected requirement signatures, y = request vectors that can
-                                  // never fit again (bit index = signature / vector id, ids >= 64 are not cached)
+  ulonglong2* pmask;              // [Cmax] per claim, by position in `order`: x = rejected requirement signatures, y = request
+                                  // vectors that can never fit again (bit index = signature / vector id, ids >= 64 are not cached)
   unsigned long long* amask;      // [Cmax] per claim: signatures that add nothing to the claim's requirements
   unsigned long long tmpl_all;    // bit n: template n survived the NewScheduler prefilter input (n < N)
   // existing-node candidate bitmaps (supersets; the exact CanAdd runs on every candidate)

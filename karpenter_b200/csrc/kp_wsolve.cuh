@@ -31,8 +31,11 @@ enum { PH_POP = 0, PH_SORT, PH_DMASK, PH_SCAN, PH_FAST, PH_RECORD, PH_EVAL, PH_N
     if (lane == 0) I.prof[p] += t_ - prof_t;  \
     prof_t = t_;                              \
   } while (0)
-#define KP_PROF_AT 16  // KpDev::counters[KP_PROF_AT + p]: cycles of phase p, then the loop's total
-#define KP_NCOUNTERS (KP_PROF_AT + KP_NPHASE + 1)
+// KpDev::counters[KP_PROF_AT + p]: cycles of phase p, then the loop's total, then the scan's steps, the positions up to
+// its results and the cycles of its first (32-wide) steps
+#define KP_PROF_AT 16
+#define KP_NPROF (KP_NPHASE + 4)
+#define KP_NCOUNTERS (KP_PROF_AT + KP_NPROF)
 #else
 #define KP_PROF_LAP(p) \
   do {                 \
@@ -68,10 +71,11 @@ struct WInst {
   int32_t* s_j;
   uint64_t* s_its;
   int32_t *order, *cnt_at;  // s.newNodeClaims: claim id / len(Pods) by position
-  // monotone failure cache, one 16-byte entry per claim: x = bit f set when requirement signature f was rejected by
-  // Requirements.Compatible, y = bit rv set when no remaining instance type can hold the claim's requests plus request
-  // vector rv.  Signatures / vectors with an index >= 64 are simply not cached (exact either way).
-  ulonglong2* cmask;
+  // monotone failure cache, one 16-byte entry per claim, stored by position like order / cnt_at (every reordering moves
+  // it), so the scan tests a position's bits without the claim id: x = bit f set when requirement signature f was
+  // rejected by Requirements.Compatible, y = bit rv set when no remaining instance type can hold the claim's requests
+  // plus request vector rv.  Signatures / vectors with an index >= 64 are simply not cached (exact either way).
+  ulonglong2* pmask;
   // amask[c] bit f: requirement signature f adds nothing to claim c's requirements.  Stable for the claim's lifetime
   // (the claim's value sets only shrink, so they stay inside the pod's), which reduces CanAdd for such a pair to the
   // resource test.
@@ -90,7 +94,7 @@ struct WInst {
   // copies can hold, 0 = not in use); the moment a claim id reaches CS everything migrates to the global arrays below.
   int CS;
   int32_t *g_order, *g_cnt_at, *g_c_tmpl;
-  ulonglong2* g_cmask;
+  ulonglong2* g_pmask;
   int64_t* tmpl_remaining;  // [N*R]
   // existing nodes
   int64_t* node_rem;
@@ -117,6 +121,7 @@ struct WInst {
   long long ev_existing, ev_inflight, ev_tmpl, commits, slow_sorts, scan_chunks, evals, fast_commits;
 #ifdef KP_PHASE_PROF
   long long prof[KP_NPHASE], prof_total;  // cycles per phase / of the whole pod loop
+  long long scan_steps, scan_pos, scan_first_cyc;  // in-flight scan: steps, positions up to each result, first-step cycles
 #endif
 };
 
@@ -258,118 +263,177 @@ struct ScanCtx {
   bool use_ez;                         // prune claims pinned to a topology-key value outside `ez` (domain_mask)
   uint64_t ez;
   const int4* hc;                      // the hostname checks: staged with the pod, or cls_hchk + hoff
+#ifdef KP_PHASE_PROF
+  long long steps, first_cyc;          // steps of the scan (first step, bit-filter steps), cycles of its first steps
+#endif
 };
-// U sub-chunks of 32 positions per step: their loads are independent, so a step costs one memory latency, not U.
-template <int U, bool LEAN = false>
-__device__ __forceinline__ int next_candidate(const KpDev& d, const WInst& I, const int32_t* ord, int nC, int from,
-                                              ScanCtx& sc, int lane, int E, int* cc_out, int limit = 0x7fffffff) {
-  const ulonglong2* cm = I.cmask;
-  if (limit > nC) limit = nC;  // positions at and above `limit` are not looked at: the caller continues there
-  for (int base = from; base < limit; base += 32 * U) {  // (unaligned: a step always looks at 32 * U fresh positions)
-    bool pass[U], fclear[U], rclear[U];
-    int c[U];
+
+// The tests of a candidate after its failure bits, ONE claim per lane (pass = the lane holds a candidate that passed its
+// bits): tolerated template, the pinned topology-key value (sc.use_ez), hostname groups.
+template <bool LEAN>
+__device__ __forceinline__ bool claim_tests(const KpDev& d, const WInst& I, const ScanCtx& sc, int c, bool pass, int E) {
+  if (pass && !sc.all_tmpl) pass = (sc.tok >> I.c_tmpl[c]) & 1ull;
+  if (!LEAN && sc.use_ez && pass) {
+    const int z = I.c_dom[c];
+    if (z != 0xff) pass = (sc.ez >> z) & 1ull;
+  }
+  // hostname groups: a NodeClaim is exactly one hostname domain (topologygroup.go:235-247,317-333,402-408).  Two
+  // groups per round, so that all their counter loads are in flight together (one L2 latency, not one per group).
+  for (int i = sc.hoff; !LEAN && i < sc.hend; i += 2) {
+    const bool two = i + 1 < sc.hend;
+    const int4 ha = sc.hc[i], hb = two ? sc.hc[i + 1] : ha;
+    // anti-affinity / affinity only ask "is the domain populated": one bit of host_pop (L1: the stager prefetched the
+    // row); a hostname spread needs the count
+    const bool cnt_a = (ha.y & 0xff) == KP_TOPO_SPREAD, cnt_b = (hb.y & 0xff) == KP_TOPO_SPREAD;
+    const int hi = E + c;
+    int ca = 0, cb = 0;
+    if (pass) {
+      ca = cnt_a ? __ldcg(d.host_cnt + (size_t)hi * d.GHS + ha.x)
+                 : (int)((d.host_pop[(size_t)ha.x * d.HW + (hi >> 5)] >> (hi & 31)) & 1u);
+      if (two)
+        cb = cnt_b ? __ldcg(d.host_cnt + (size_t)hi * d.GHS + hb.x)
+                   : (int)((d.host_pop[(size_t)hb.x * d.HW + (hi >> 5)] >> (hi & 31)) & 1u);
+    }
 #pragma unroll
-    for (int u = 0; u < U; u++) {
+    for (int r = 0; r < 2; r++) {
+      if (r == 1 && !two) break;
+      const int4 hc = r == 0 ? ha : hb;
+      const int type = hc.y & 0xff, self = hc.y >> 8;
+      if (!pass) continue;
+      const int hcnt = r == 0 ? ca : cb;
+      if (type == KP_TOPO_SPREAD)
+        pass = hcnt + self <= hc.z;
+      else if (type == KP_TOPO_AFFINITY)
+        pass = hcnt > 0 || (self && (d.g_ndomains[hc.w] - d.g_nempty[hc.w]) == 0);
+      else
+        pass = hcnt == 0;
+    }
+  }
+  return pass;
+}
+
+// the scan bounds: the first position with a clear signature / request-vector bit, from the bit tests of the 32
+// positions b .. b+31 (lane order is position order)
+__device__ __forceinline__ void scan_clear(ScanCtx& sc, int b, bool fclear, bool rclear) {
+  if (sc.fbit && sc.first_clear < 0) {
+    const unsigned fm = __ballot_sync(FULL, fclear);
+    if (fm) sc.first_clear = b + __ffs(fm) - 1;
+  }
+  if (sc.rbit && sc.first_rclear < 0) {
+    const unsigned rm = __ballot_sync(FULL, rclear);
+    if (rm) sc.first_rclear = b + __ffs(rm) - 1;
+  }
+}
+
+// position of the n-th (from 0) set bit of m; m has more than n bits set
+__device__ __forceinline__ int nth_bit(unsigned m, int n) {
+  int p = 0;
+#pragma unroll
+  for (int w = 16; w; w >>= 1) {
+    const int k = __popc(m & ((1u << w) - 1u));
+    if (n >= k) {
+      n -= k;
+      m >>= w;
+      p += w;
+    }
+  }
+  return p;
+}
+
+// The in-flight scan.  The first step takes the 32 positions from `from`, one per lane, through every test: most pods
+// find their claim there.  Each later step is two-level.  Level 1 tests only the failure bits of 256 positions, 8 per
+// lane strided by 32 so that ballot order is position order: their pmask loads are independent, so a step in which
+// every claim is dead costs one memory latency.  Level 2 packs the survivors into lanes in position order, 32 at a time,
+// and runs the claim tests on them.  Either way the result is the lowest position >= `from` that passes every test.
+#define KP_SCAN_L1 8  // level-1 positions per lane
+template <bool LEAN>
+__device__ __forceinline__ int next_candidate(const KpDev& d, const WInst& I, const int32_t* ord, int nC, int from,
+                                              ScanCtx& sc, int lane, int E, int* cc_out) {
+  const ulonglong2* pm = I.pmask;
+#ifdef KP_PHASE_PROF
+  const long long t0 = clock64();
+  sc.steps++;
+#endif
+  {
+    const int pos = from + lane;
+    int c = -1;
+    bool fclear = false, rclear = false;
+    if (pos < nC) {
+      c = ord[pos];
+      const ulonglong2 mk = pm[pos];
+      fclear = !(mk.x & sc.fbit);
+      rclear = !(mk.y & sc.rbit);
+    }
+    scan_clear(sc, from, fclear, rclear);
+    const unsigned m = __ballot_sync(FULL, claim_tests<LEAN>(d, I, sc, c, fclear && rclear, E));
+#ifdef KP_PHASE_PROF
+    sc.first_cyc += clock64() - t0;
+#endif
+    if (m) {
+      const int l = __ffs(m) - 1;
+      *cc_out = __shfl_sync(FULL, c, l);
+      return from + l;
+    }
+  }
+  for (int base = from + 32; base < nC; base += 32 * KP_SCAN_L1) {
+#ifdef KP_PHASE_PROF
+    sc.steps++;
+#endif
+    bool fclear[KP_SCAN_L1], rclear[KP_SCAN_L1];
+#pragma unroll
+    for (int u = 0; u < KP_SCAN_L1; u++) {
       const int pos = base + u * 32 + lane;
-      c[u] = -1;
-      pass[u] = fclear[u] = rclear[u] = false;
-      if (pos < limit && pos >= from) {
-        c[u] = ord[pos];
-        const ulonglong2 mk = cm[c[u]];
+      fclear[u] = rclear[u] = false;
+      if (pos < nC) {
+        const ulonglong2 mk = pm[pos];
         fclear[u] = !(mk.x & sc.fbit);
         rclear[u] = !(mk.y & sc.rbit);
-        pass[u] = fclear[u] && rclear[u];
-        if (pass[u] && !sc.all_tmpl) pass[u] = (sc.tok >> I.c_tmpl[c[u]]) & 1ull;
       }
     }
-    if (!LEAN && sc.use_ez) {
+    unsigned sm[KP_SCAN_L1];  // survivors of sub-step u
+    int pre[KP_SCAN_L1];      // survivors before sub-step u
+    int S = 0;
 #pragma unroll
-      for (int u = 0; u < U; u++)
-        if (pass[u]) {
-          const int z = I.c_dom[c[u]];
-          if (z != 0xff) pass[u] = (sc.ez >> z) & 1ull;
-        }
+    for (int u = 0; u < KP_SCAN_L1; u++) {
+      scan_clear(sc, base + u * 32, fclear[u], rclear[u]);
+      sm[u] = __ballot_sync(FULL, fclear[u] && rclear[u]);
+      pre[u] = S;
+      S += __popc(sm[u]);
     }
-    // hostname groups: a NodeClaim is exactly one hostname domain (topologygroup.go:235-247,317-333,402-408).  Two
-    // groups per round, so that all their counter loads are in flight together (one L2 latency, not one per group).
-    for (int i = sc.hoff; !LEAN && i < sc.hend; i += 2) {
-      const bool two = i + 1 < sc.hend;
-      const int4 ha = sc.hc[i], hb = two ? sc.hc[i + 1] : ha;
-      // anti-affinity / affinity only ask "is the domain populated": one bit of host_pop (L1: the stager prefetched the
-      // row); a hostname spread needs the count
-      const bool cnt_a = (ha.y & 0xff) == KP_TOPO_SPREAD, cnt_b = (hb.y & 0xff) == KP_TOPO_SPREAD;
-      int ca[U], cb[U];
+    for (int b = 0; b < S; b += 32) {
+      const int r = b + lane;  // this lane takes survivor r
+      int pos = -1, c = -1;
+      if (r < S) {
+        unsigned mu = sm[0];
+        int ru = r, uo = 0;
 #pragma unroll
-      for (int u = 0; u < U; u++) {
-        const int hi = E + c[u];
-        ca[u] = cb[u] = 0;
-        if (pass[u]) {
-          ca[u] = cnt_a ? __ldcg(d.host_cnt + (size_t)hi * d.GHS + ha.x)
-                        : (int)((d.host_pop[(size_t)ha.x * d.HW + (hi >> 5)] >> (hi & 31)) & 1u);
-          if (two)
-            cb[u] = cnt_b ? __ldcg(d.host_cnt + (size_t)hi * d.GHS + hb.x)
-                          : (int)((d.host_pop[(size_t)hb.x * d.HW + (hi >> 5)] >> (hi & 31)) & 1u);
-        }
+        for (int u = 1; u < KP_SCAN_L1; u++)
+          if (r >= pre[u]) {
+            mu = sm[u];
+            ru = r - pre[u];
+            uo = u * 32;
+          }
+        pos = base + uo + nth_bit(mu, ru);
+        c = ord[pos];
       }
-#pragma unroll
-      for (int r = 0; r < 2; r++) {
-        if (r == 1 && !two) break;
-        const int4 hc = r == 0 ? ha : hb;
-        const int type = hc.y & 0xff, self = hc.y >> 8;
-#pragma unroll
-        for (int u = 0; u < U; u++) {
-          if (!pass[u]) continue;
-          const int hcnt = r == 0 ? ca[u] : cb[u];
-          if (type == KP_TOPO_SPREAD)
-            pass[u] = hcnt + self <= hc.z;
-          else if (type == KP_TOPO_AFFINITY)
-            pass[u] = hcnt > 0 || (self && (d.g_ndomains[hc.w] - d.g_nempty[hc.w]) == 0);
-          else
-            pass[u] = hcnt == 0;
-        }
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      if (sc.fbit && sc.first_clear < 0) {
-        const unsigned fm = __ballot_sync(FULL, fclear[u]);
-        if (fm) sc.first_clear = base + u * 32 + __ffs(fm) - 1;
-      }
-      if (sc.rbit && sc.first_rclear < 0) {
-        const unsigned rm = __ballot_sync(FULL, rclear[u]);
-        if (rm) sc.first_rclear = base + u * 32 + __ffs(rm) - 1;
-      }
-      const unsigned m = __ballot_sync(FULL, pass[u]);
+      const unsigned m = __ballot_sync(FULL, claim_tests<LEAN>(d, I, sc, c, r < S, E));
       if (m) {
         const int l = __ffs(m) - 1;
-        *cc_out = __shfl_sync(FULL, c[u], l);
-        return base + u * 32 + l;
+        *cc_out = __shfl_sync(FULL, c, l);
+        return __shfl_sync(FULL, pos, l);
       }
     }
   }
   return -1;
 }
 
-// The cheap tests of next_candidate for ONE claim per lane, without the topology-key mask (which changes from pod to pod
-// of a cohort): failure bits, tolerated template, hostname groups.
+// The cheap tests of next_candidate for ONE claim per lane (mk: its failure masks), without the topology-key mask (which
+// changes from pod to pod of a cohort): failure bits, tolerated template, hostname groups.
 template <bool LEAN>
-__device__ __forceinline__ bool cheap_pass(const KpDev& d, const WInst& I, const ScanCtx& sc, int c, int E) {
-  const ulonglong2 mk = I.cmask[c];
-  bool pass = !(mk.x & sc.fbit) && !(mk.y & sc.rbit);
-  if (pass && !sc.all_tmpl) pass = (sc.tok >> I.c_tmpl[c]) & 1ull;
-  for (int i = sc.hoff; !LEAN && pass && i < sc.hend; i++) {
-    const int4 hc = sc.hc[i];
-    const int type = hc.y & 0xff, self = hc.y >> 8, hi = E + c;
-    const int hcnt = type == KP_TOPO_SPREAD ? __ldcg(d.host_cnt + (size_t)hi * d.GHS + hc.x)
-                                            : (int)((d.host_pop[(size_t)hc.x * d.HW + (hi >> 5)] >> (hi & 31)) & 1u);
-    if (type == KP_TOPO_SPREAD)
-      pass = hcnt + self <= hc.z;
-    else if (type == KP_TOPO_AFFINITY)
-      pass = hcnt > 0 || (self && (d.g_ndomains[hc.w] - d.g_nempty[hc.w]) == 0);
-    else
-      pass = hcnt == 0;
-  }
-  return pass;
+__device__ __forceinline__ bool cheap_pass(const KpDev& d, const WInst& I, const ScanCtx& sc, int c, ulonglong2 mk, int E) {
+  ScanCtx st = sc;
+  st.use_ez = false;
+  return claim_tests<LEAN>(d, I, st, c, !(mk.x & sc.fbit) && !(mk.y & sc.rbit), E);
 }
 
 // CanAdd of k more pods of the staged class on a claim whose requirements they leave as they are (the "adds nothing" fast
@@ -416,7 +480,7 @@ __device__ __forceinline__ void migrate_small(const KpDev& d, WInst& I, int nC, 
     I.g_order[i] = I.order[i];
     I.g_cnt_at[i] = I.cnt_at[i];
     I.g_c_tmpl[i] = I.c_tmpl[i];
-    I.g_cmask[i] = I.cmask[i];
+    I.g_pmask[i] = I.pmask[i];
     I.g_amask[i] = I.amask[i];
     if (I.c_dom) I.g_c_dom[i] = I.c_dom[i];
   }
@@ -425,7 +489,7 @@ __device__ __forceinline__ void migrate_small(const KpDev& d, WInst& I, int nC, 
     I.order = I.g_order;
     I.cnt_at = I.g_cnt_at;
     I.c_tmpl = I.g_c_tmpl;
-    I.cmask = I.g_cmask;
+    I.pmask = I.g_pmask;
     I.amask = I.g_amask;
     if (I.c_dom) I.c_dom = I.g_c_dom;
     I.CS = 0;
@@ -574,15 +638,16 @@ __device__ __noinline__ CohortOut cohort_try(const KpDev& d, WInst& I, const Pod
     st.first_clear = 0;
     st.first_rclear = 0;
     int c2;
-    w0 = st.hend > st.hoff ? next_candidate<4, LEAN>(d, I, ord, nC, lb, st, lane, E, &c2)
-                           : next_candidate<1, LEAN>(d, I, ord, nC, lb, st, lane, E, &c2);
+    w0 = next_candidate<LEAN>(d, I, ord, nC, lb, st, lane, E, &c2);
     if (w0 < 0 || w0 > cpos) w0 = cpos;
   }
   const int pw = w0 + lane;
   int wc = -1, wn = -1;
+  ulonglong2 wp = make_ulonglong2(0ull, 0ull);
   if (pw < nC) {
     wc = ord[pw];
     wn = cnt[pw];
+    wp = I.pmask[pw];
   }
   const int c0 = __shfl_sync(FULL, wn, 0);
   const unsigned gmask = __ballot_sync(FULL, pw < nC && wn == c0);
@@ -616,7 +681,7 @@ __device__ __noinline__ CohortOut cohort_try(const KpDev& d, WInst& I, const Pod
       k = good;
     }
     if (k == 0) {  // not even one: permanent for this request vector
-      if (lane == 0) I.cmask[cc].y |= rbit;
+      if (lane == 0) I.pmask[cpos].y |= rbit;
       __syncwarp();
       out.state = 1;
       return out;
@@ -640,7 +705,7 @@ __device__ __noinline__ CohortOut cohort_try(const KpDev& d, WInst& I, const Pod
   bool wpass = false, wfp = false;
   int wz = -1;
   if (lane < gsz) {
-    wpass = cheap_pass<LEAN>(d, I, sc, wc, E);
+    wpass = cheap_pass<LEAN>(d, I, sc, wc, wp, E);
     if (wpass) {
       wfp = (I.amask[wc] & abit) != 0;
       if (wfp && !fast_ok && has_tk) {
@@ -694,7 +759,9 @@ __device__ __noinline__ CohortOut cohort_try(const KpDev& d, WInst& I, const Pod
     out.nevals++;
     avail &= ~(1u << l);
     if (!fp_fit(d, I, px, cl, 1, lane, &q, &lo, &adv, &its)) {  // full: the same pod takes the next claim
-      if (lane == 0) I.cmask[cl].y |= rbit;
+      // (nothing has moved yet: the claim still stands at w0 + l, and lane l carries its masks to where it ends up)
+      if (lane == 0) I.pmask[w0 + l].y |= rbit;
+      if (lane == l) wp.y |= rbit;
       __syncwarp();
       continue;
     }
@@ -727,12 +794,14 @@ __device__ __noinline__ CohortOut cohort_try(const KpDev& d, WInst& I, const Pod
       const int i = s0 + lane;
       const bool in = i < nC && cnt[i] == c0;
       const int vo = in ? ord[i] : 0;
+      const ulonglong2 vp = in ? I.pmask[i] : make_ulonglong2(0ull, 0ull);
       const unsigned gk = __ballot_sync(FULL, in);
       const int n = gk == FULL ? 32 : __ffs(~gk) - 1;
       __syncwarp();
       if (lane < n) {
         ord[i - m] = vo;
         cnt[i - m] = c0;
+        I.pmask[i - m] = vp;
       }
       __syncwarp();
       gE = s0 + n - 1;
@@ -743,13 +812,10 @@ __device__ __noinline__ CohortOut cohort_try(const KpDev& d, WInst& I, const Pod
   const int rank = __popc(~picked & ((1u << lane) - 1));  // claims below me that stay
   __syncwarp();
   if (lane < gsz) {
-    if (mv) {
-      ord[gE - my_t] = wc;
-      cnt[gE - my_t] = c0 + 1;
-    } else {
-      ord[w0 + rank] = wc;
-      cnt[w0 + rank] = lane == prev_l ? c0 + 1 : c0;
-    }
+    const int to = mv ? gE - my_t : w0 + rank;
+    ord[to] = wc;
+    cnt[to] = mv || lane == prev_l ? c0 + 1 : c0;
+    I.pmask[to] = wp;
   }
   __syncwarp();
   out.state = 2;
@@ -837,8 +903,10 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
 #ifdef KP_PHASE_PROF
   long long prof_t = clock64();
   const long long prof_t0 = prof_t;
-  if (lane == 0)
+  if (lane == 0) {
     for (int p = 0; p < KP_NPHASE; p++) I.prof[p] = 0;
+    I.scan_steps = I.scan_pos = I.scan_first_cyc = 0;
+  }
 #endif
   for (;;) {
     KP_PROF_LAP(PH_OTHER);
@@ -1074,20 +1142,24 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
           const int q4 = nC / 4;
           stable = pert == PERT_APPEND || !(p == q4 - 1 || p == q4 || p == 2 * q4 - 1 || p == 2 * q4 || p == 3 * q4 - 1 || p == 3 * q4);
         }
+        ulonglong2* const pm = I.pmask;  // moves with the order
         if (stable) {
           if (pert == PERT_INC) {  // elevated count: shift smaller successors left until one is not smaller
             const int ec = cnt[p], eo = ord[p];
+            const ulonglong2 ep = pm[p];
             int i0 = p;
             for (;;) {
               const int i = i0 + lane;
               const bool in = i + 1 < nC;
               const int vc = in ? cnt[i + 1] : 0x7fffffff, vo = in ? ord[i + 1] : 0;
+              const ulonglong2 vp = in ? pm[i + 1] : ep;
               const unsigned stop = __ballot_sync(FULL, vc >= ec);
               const int nmove = stop ? __ffs(stop) - 1 : 32;
               __syncwarp();
               if (lane < nmove) {
                 cnt[i] = vc;
                 ord[i] = vo;
+                pm[i] = vp;
               }
               __syncwarp();
               i0 += nmove;
@@ -1096,6 +1168,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
             if (lane == 0) {
               cnt[i0] = ec;
               ord[i0] = eo;
+              pm[i0] = ep;
             }
             // positions (p, i0] moved one to the left: a bound inside that range follows its elements
             if (p < lb0 && lb0 <= i0) lb0--;
@@ -1104,17 +1177,20 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
             if (p < lr1 && lr1 <= i0) lr1--;
           } else {  // new claim appended: shift larger predecessors right until one is not larger
             const int ec = cnt[nC - 1], eo = ord[nC - 1];
+            const ulonglong2 ep = pm[nC - 1];
             int i0 = nC - 1;
             for (;;) {
               const int i = i0 - lane;
               const bool in = i - 1 >= 0;
               const int vc = in ? cnt[i - 1] : -0x7fffffff, vo = in ? ord[i - 1] : 0;
+              const ulonglong2 vp = in ? pm[i - 1] : ep;
               const unsigned stop = __ballot_sync(FULL, vc <= ec);
               const int nmove = stop ? __ffs(stop) - 1 : 32;
               __syncwarp();
               if (lane < nmove) {
                 cnt[i] = vc;
                 ord[i] = vo;
+                pm[i] = vp;
               }
               __syncwarp();
               i0 -= nmove;
@@ -1123,6 +1199,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
             if (lane == 0) {
               cnt[i0] = ec;
               ord[i0] = eo;
+              pm[i0] = ep;
             }
             // the new claim (untested by every signature) now sits at i0
             if (lb0 > i0) lb0 = i0;
@@ -1132,7 +1209,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
           }
         } else {
           // exact pdqsort emulation (rare: ties scrambled by Go's unstable partition), warp-cooperative
-          WarpSorter s{cnt, ord, lane};
+          WarpSorterT<int, true> s{cnt, ord, lane, pm};
           s.pdqsort(0, nC, WarpSorter::bits_len((unsigned long long)nC));
           slow_sorts++;
           lb0 = 0;  // ties were permuted arbitrarily: the bounds restart
@@ -1162,6 +1239,10 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
       sc.first_rclear = -1;
       sc.use_ez = false;
       sc.ez = ~0ull;
+#ifdef KP_PHASE_PROF
+      sc.steps = 0;
+      sc.first_cyc = 0;
+#endif
       // tkinfo (host-computed per class, kp_prep.cpp plan_classes): which shortcuts the class may take
       const int tki = px.tkinfo;
       // bit of the pod's requirement set in the claims' "adds nothing" masks
@@ -1210,16 +1291,10 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
         if ((sc.hc[i].y & 0xff) == KP_TOPO_AFFINITY) coh_ok = false;  // "is any domain populated" changes with every record
       while (scanned && !found) {
         int cc;
-        // classes with hostname checks read presence words / counters per candidate: 128 positions per step there (their
-        // loads overlap) -- after ONE 32-wide step: most pods find their claim among the first positions of the scan
-        int cpos;
-        if (sc.hend > sc.hoff) {
-          const int lim = from + 32;
-          cpos = next_candidate<1, LEAN>(d, I, ord, nC, from, sc, lane, E, &cc, lim);
-          if (cpos < 0 && lim < nC) cpos = next_candidate<4, LEAN>(d, I, ord, nC, lim, sc, lane, E, &cc);
-        } else {
-          cpos = next_candidate<1, LEAN>(d, I, ord, nC, from, sc, lane, E, &cc);
-        }
+        const int cpos = next_candidate<LEAN>(d, I, ord, nC, from, sc, lane, E, &cc);
+#ifdef KP_PHASE_PROF
+        if (lane == 0) I.scan_pos += (cpos < 0 ? nC : cpos + 1) - from;
+#endif
         KP_PROF_LAP(PH_SCAN);
         if (cpos < 0) break;
         from = cpos + 1;
@@ -1263,7 +1338,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
             const bool ok = fp_fit(d, I, px, cc, 1, lane, &q, &lo, &any_adv, &its);
             evals++;
             if (!ok) {  // nothing left that holds the merged requests: permanent for this request vector
-              if (lane == 0) I.cmask[cc].y |= rbit;
+              if (lane == 0) I.pmask[cpos].y |= rbit;
               __syncwarp();
               KP_PROF_LAP(PH_FAST);
               continue;
@@ -1322,10 +1397,10 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
           if (VOL && alt_loaded && !ev.ok) load_alt_slots(d, pxw, Xc, lane);  // the next candidate starts with the first alternative
           if (!ev.ok) {
             if (lane == 0) {
-              ulonglong2 mk = I.cmask[cc];
+              ulonglong2 mk = I.pmask[cpos];
               if (ev.res_dead) mk.y |= rbit;
               if (ev.compat_fail) mk.x |= fbit;
-              I.cmask[cc] = mk;
+              I.pmask[cpos] = mk;
             }
             __syncwarp();
             KP_PROF_LAP(PH_EVAL);
@@ -1355,6 +1430,12 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
           found = true;
         }
       }
+#ifdef KP_PHASE_PROF
+      if (lane == 0) {
+        I.scan_steps += sc.steps;
+        I.scan_first_cyc += sc.first_cyc;
+      }
+#endif
       // a bound may only advance when the scan really started at it (positions below `lb` were not looked at)
       if (fbit && scanned && lbf == lb) {  // all positions below the first clear bit rejected the signature
         const int nb = sc.first_clear >= 0 ? sc.first_clear : nC;
@@ -1487,9 +1568,9 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
           I.pod_error[li] = KP_PODERR_NONE;
         }
       }
-      // a recycled instance must not inherit failure bits of an earlier claim with this id
+      // a recycled instance must not inherit failure bits of an earlier claim at this position
       if (lane == 0) {
-        I.cmask[cnew] = make_ulonglong2(0ull, 0ull);
+        I.pmask[cnew] = make_ulonglong2(0ull, 0ull);
         I.amask[cnew] = ((px.tkinfo & TKI_ABIT) && ev.pod_noop) ? 1ull << (px.tkinfo & 63) : 0ull;
         if (!LEAN && d.n_rsv) I.c_rsv[cnew] = take;
         if (!LEAN && d.n_hostports) I.c_ports[cnew] = d.tmpl_ports[n] | px.ports;

@@ -21,6 +21,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 PHASES = ["pop", "sort", "domain_mask", "scan", "fast_commit", "record", "full_eval", "new_claim", "other"]
+# the in-flight scan's counters: steps (the first 32-wide step, each later step), positions from the scan start up to each
+# result (what a position-by-position walk visits), cycles of the first steps (the rest of the scan phase: later steps)
+SCAN = ["steps", "positions", "first_step_cycles"]
 
 
 def gpu_info():
@@ -37,18 +40,21 @@ def profile(h, lib, problem, n_pods):
     h.solve_resident()  # warm-up
     res = h.solve_resident()
     st = h.stats()
-    buf = np.zeros(len(PHASES) + 1, dtype=np.int64)
+    buf = np.zeros(len(PHASES) + 1 + len(SCAN), dtype=np.int64)
     n = lib.kp_phase_profile(h._h, -1, buf.ctypes.data_as(C.c_void_p), len(buf))
     if n != len(buf):
         raise RuntimeError("kp_phase_profile failed: is KP_LIB_PATH the profiling build (libkarpsolve_prof.so)?")
     per_pod = {p: float(buf[i]) / n_pods for i, p in enumerate(PHASES)}
+    scan = {s: float(buf[len(PHASES) + 1 + i]) / n_pods for i, s in enumerate(SCAN)}
+    scan["later_step_cycles"] = per_pod["scan"] - scan["first_step_cycles"]
     return {
         "pods": n_pods,
         "claims": int(res["n_claims"]),
         "solve_ms": st["solve_ms"],
         "cycles_per_pod": per_pod,
-        "sum_cycles_per_pod": float(buf[:-1].sum()) / n_pods,
-        "total_cycles_per_pod": float(buf[-1]) / n_pods,
+        "sum_cycles_per_pod": float(buf[:len(PHASES)].sum()) / n_pods,
+        "total_cycles_per_pod": float(buf[len(PHASES)]) / n_pods,
+        "scan_per_pod": scan,
     }
 
 
@@ -80,6 +86,9 @@ def main():
             c = r["cycles_per_pod"][p]
             print(f"  {p:12s} {c:9.1f} cycles/pod  {100 * c / r['total_cycles_per_pod']:5.1f} %")
         print(f"  {'sum':12s} {r['sum_cycles_per_pod']:9.1f}   total {r['total_cycles_per_pod']:.1f} cycles/pod")
+        s = r["scan_per_pod"]
+        print(f"  scan: {s['steps']:.2f} steps/pod, {s['positions']:.1f} positions/pod, first steps "
+              f"{s['first_step_cycles']:.1f} cycles/pod, later steps {s['later_step_cycles']:.1f} cycles/pod")
     if args.json:
         with open(args.json, "w") as f:
             json.dump(out, f, indent=1)
