@@ -522,8 +522,7 @@ static int upload_tables(kp_handle* h, Instance& in, const kp_problem* p, int cm
   CK(up_mut(h, in, &d.g_birth, t.g_birth));
   CK(up(h, &d.cls_lazy_off, t.cls_lazy_off));
   CK(up(h, &d.cls_lazy, t.cls_lazy));
-  CK(up_mut(h, in, &d.g_ndomains, t.g_ndomains));
-  CK(up_mut(h, in, &d.g_nempty, t.g_nempty));
+  CK(up_mut(h, in, &d.g_anypop, t.g_anypop));
   CK(up(h, &d.node_taintset, t.node_taintset));
   CK(up(h, &d.node_flags, t.node_flags));
   CK(up_mut(h, in, &d.node_rem, t.node_rem));

@@ -205,16 +205,14 @@ __device__ __forceinline__ Slot topo_domains(const KpDev& d, int g, const KpGrou
   return out;
 }
 
-// TopologyGroup.Record on a hostname group (topologygroup.go:141-155): one more pod of the group on `host`.  The
-// presence bit answers "was the domain empty" from L1; the counter itself is a fire-and-forget reduction.
+// TopologyGroup.Record on a hostname group (topologygroup.go:141-155): one more pod of the group on `host`.  Nothing
+// here needs to know whether the domain was empty (g_anypop is only ever set), so the record is write-only: two
+// fire-and-forget reductions and a store, no load on the solver's chain.  The owning warp is the only writer, and a
+// __syncwarp lies between every record and the warp's next read of these tables, which orders the two.
 __device__ __forceinline__ void host_record(const KpDev& d, int row, int g, int host) {
-  uint32_t* w = d.host_pop + (size_t)row * d.HW + (host >> 5);
-  const uint32_t bit = 1u << (host & 31), cur = *w;
-  if (!(cur & bit)) {
-    *w = cur | bit;
-    d.g_nempty[g]--;
-  }
+  atomicOr(d.host_pop + (size_t)row * d.HW + (host >> 5), 1u << (host & 31));
   atomicAdd(d.host_cnt + (size_t)host * d.GHS + row, 1);
+  d.g_anypop[g] = 1;
 }
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 
@@ -338,7 +336,7 @@ __device__ __forceinline__ Eval eval_candidate(const KpDev& d, const PodCtx& px,
           if (G.type == KP_TOPO_SPREAD)
             ok = cnt + (self ? 1 : 0) <= G.max_skew;
           else if (G.type == KP_TOPO_AFFINITY)
-            ok = cnt > 0 || (self && (d.g_ndomains[g] - d.g_nempty[g]) == 0);
+            ok = cnt > 0 || (self && d.g_anypop[g] == 0);
           else
             ok = cnt == 0;
           if (!ok) fail = true;

@@ -978,6 +978,7 @@ int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
   h.groups.resize(std::max(G, 1));
   h.dom_reg.assign(std::max(G, 1), 0);
   h.dom_pop.assign(std::max(G, 1), 0);
+  h.g_anypop.assign(std::max(G, 1), 0);
   h.g_ndomains.assign(std::max(G, 1), 0);
   h.g_nempty.assign(std::max(G, 1), 0);
   h.dom_cnt.assign((size_t)std::max(G, 1) * 64, 0);
@@ -998,16 +999,13 @@ int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
       int pop = 0;
       for (auto& kv : g.host_cnt) pop += kv.second > 0;
       h.g_nempty[gi] = (int)g.host_reg.size() - pop;
+      h.g_anypop[gi] = pop > 0;
     } else {
       h.dom_reg[gi] = g.reg;
       for (int v = 0; v < 64; v++) {
         h.dom_cnt[(size_t)gi * 64 + v] = g.cnt[v];
         if (g.cnt[v] > 0) h.dom_pop[gi] |= 1ull << v;
       }
-      h.g_ndomains[gi] = __builtin_popcountll(g.reg);
-      int pop = 0;
-      for (int v = 0; v < 64; v++) pop += (g.reg >> v & 1) && g.cnt[v] > 0;
-      h.g_nempty[gi] = h.g_ndomains[gi] - pop;
     }
     h.groups[gi] = g.g;
   }

@@ -91,7 +91,8 @@ struct HostTables {
   std::vector<int32_t> filter_rs;
   std::vector<int32_t> dom_cnt;
   std::vector<uint64_t> dom_reg, dom_pop;
-  std::vector<int32_t> g_ndomains, g_nempty;
+  std::vector<int32_t> g_anypop;               // hostname groups: KpDev::g_anypop
+  std::vector<int32_t> g_ndomains, g_nempty;   // hostname groups: len(t.domains), len(t.emptyDomains) (the cached CPU solver)
   std::vector<int32_t> host_cnt_nodes;  // [GH * E] initial hostname-group counts of existing nodes
   std::vector<int32_t> node_taintset;
   std::vector<uint8_t> node_flags;

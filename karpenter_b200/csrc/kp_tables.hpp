@@ -151,8 +151,15 @@ struct KpDev {
   uint64_t *tk_reg, *tk_pop;
   int32_t* tk_cnt;
   int tk_nv;                      // value ids of tk_key lie below this
-  int32_t* g_ndomains;            // [G] hostname groups: len(t.domains)
-  int32_t* g_nempty;              // [G] hostname groups: len(t.emptyDomains)
+  // the domain fast path (kp_kernels.cuh domain_mask): the one non-hostname key topology groups of fast-path classes
+  // use (-1: none), and per claim the value its slot on that key is pinned to (0xff: not a single In value)
+  int tk_key;
+  uint8_t* c_dom;                 // [Cmax]
+  int32_t* g_anypop;              // [G] hostname groups: some domain is populated (len(t.domains) > len(t.emptyDomains)).
+                                  // Only ever set during a solve (Record populates, Register adds empty domains, nothing
+                                  // unregisters), so a record sets it with a plain store and reads nothing
+  // (tk_key and c_dom sit here so that every field below stays 16-byte aligned as it is: k_wsolve_batch reads this block
+  // from shared memory in 16-byte pairs, and its register count moves with that pairing)
   int32_t* host_cnt;              // [H * GHS] HOST-major (existing nodes then claims), GHS = max(GH, 1) ints per host: only
                                   // the rows of hosts that exist are ever touched, so the footprint (and the TLB reach it
                                   // needs) follows the NodeClaims opened, not the capacity provisioned for them.
@@ -230,9 +237,5 @@ struct KpDev {
   unsigned long long* c_rsv;      // [Cmax]
   int rsv_ct_key, rsv_reserved_val, rsv_id_key;  // FinalizeScheduling's pins (nodeclaim.go:291-307)
   unsigned long long rsv_val_of[64];             // value bit (in rsv_id_key) of reservation id i
-  // the domain fast path (kp_kernels.cuh domain_mask): the one non-hostname key topology groups of fast-path classes
-  // use (-1: none), and per claim the value its slot on that key is pinned to (0xff: not a single In value)
-  int tk_key;
-  uint8_t* c_dom;                 // [Cmax]
   long long deadline_ns;          // 0 = none; the solve stops with KP_DEADLINE once this much device time has passed
 };

@@ -304,7 +304,7 @@ __device__ __forceinline__ bool claim_tests(const KpDev& d, const WInst& I, cons
       if (type == KP_TOPO_SPREAD)
         pass = hcnt + self <= hc.z;
       else if (type == KP_TOPO_AFFINITY)
-        pass = hcnt > 0 || (self && (d.g_ndomains[hc.w] - d.g_nempty[hc.w]) == 0);
+        pass = hcnt > 0 || (self && d.g_anypop[hc.w] == 0);
       else
         pass = hcnt == 0;
     }
@@ -1595,15 +1595,8 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
           if (lane == 0) I.tmpl_remaining[(size_t)n * R + r] -= mx;
         }
       }
-      // Topology.Register(hostname) (nodeclaim.go:213): every hostname group learns the new, empty domain
-      if (!LEAN && d.GH > 0) {
-        for (int g = lane; g < d.G; g += 32)
-          if (d.groups[g].key == d.hostname_key) {
-            d.g_ndomains[g]++;
-            d.g_nempty[g]++;
-          }
-        __syncwarp();
-      }
+      // Topology.Register(hostname) (nodeclaim.go:213) adds the new, empty domain to every hostname group.  The device
+      // keeps only whether a group has a populated domain (g_anypop), which an empty domain does not change: nothing to do.
       if (!LEAN) topo_record(d, px, ev.F, d.tmpl_taintset[n], E + cnew, true, lane);
       __syncwarp();
       nC = cnew + 1;
