@@ -37,7 +37,9 @@ typedef enum kp_status {
   KP_ERR_INVALID = 2,      /* malformed problem */
   KP_ERR_CUDA = 3,         /* device / driver failure; message via kp_last_error */
   KP_ERR_CAPACITY = 4,     /* a compiled limit was exceeded (e.g. > KP_MAX_RESOURCES) */
-  KP_ERR_UNSUPPORTED = 5   /* feature of the reference not built yet (CSI volume limits, BestEffort minValues in kp_consolidate) */
+  KP_ERR_UNSUPPORTED = 5   /* feature of the reference not built yet (CSI volume limits, BestEffort minValues in kp_consolidate,
+                              kubernetes.io/hostname on a NodePool / instance type / offering, with Gt / Lt / minValues, or
+                              together with hostname-key pod affinity) */
 } kp_status;
 
 /* ---- requirement encoding --------------------------------------------------------------------------------------

@@ -399,6 +399,7 @@ static int upload_tables(kp_handle* h, Instance& in, const kp_problem* p, int cm
   CK(up(h, &d.tmpl_daemon, t.tmpl_daemon));
   CK(up_mut(h, in, &d.tmpl_remaining, t.tmpl_remaining));
   CK(up(h, &d.tmpl_limit_present, t.tmpl_limit_present));
+  CK(up(h, &d.host_rules, t.host_rules));
   CK(up(h, &d.cls_req, t.cls_req));
   CK(up(h, &d.cls_rs, t.cls_rs));
   CK(up(h, &d.cls_tolset, t.cls_tolset));
@@ -752,7 +753,7 @@ static int add_instance(kp_handle* h, const kp_problem* p, int64_t cmax) {
   std::vector<uint8_t> active(p->n_nodes, 0);
   for (int i = 0; i < p->n_nodes; i++) active[i] = (p->node_flags[i] & KP_NODE_SCHEDULABLE) != 0;
   std::vector<int32_t> pending(p->pod_class, p->pod_class + p->n_pods);
-  int rc = kp_prepare(p, active, {}, pending, in.host, h->err);
+  int rc = kp_prepare(p, active, {}, pending, in.host, h->err, true);
   if (rc != KP_OK) return rc;
   auto t1 = std::chrono::steady_clock::now();
   h->stats.prep_ms += std::chrono::duration<double, std::milli>(t1 - t0).count();
@@ -1751,6 +1752,9 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   KpDev dq = d;  // the cluster's pointer block with k_consolidate's table plan (the upload keeps the solver's)
   dq.tab_bytes = plan_tables(dq, fixed, budget);
   const size_t smem = fixed + dq.tab_bytes + 64;
+  if (getenv("KP_DEBUG"))
+    fprintf(stderr, "[kp] consolidate plan: tables %zu B staged of %zu B, %zu B shared\n", (size_t)dq.tab_bytes,
+            kp_tab_bytes(dq), smem);
   const bool lean = !t.has_bounds && !t.min_values_strict && t.n_rsv == 0 && d.n_hostports == 0 && !getenv("KP_NO_LEAN");  // (G == 0 here)
   CK(cudaFuncSetAttribute(lean ? k_consolidate<true> : k_consolidate<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int per_sm = 1;

@@ -89,6 +89,7 @@ __global__ void __launch_bounds__(256) k_node_cand(KpDev d, const int32_t* nsig_
     if (row < d.n_nsig) {
       bit = tolerated(d, nsig_tolset[row], d.node_taintset[n]);
       const int rs = nsig_rs[row];  // -1: a class with volume-topology alternatives -- every tolerated node is a candidate
+      if (rs >= 0 && bit) bit = host_rule_admits(d.host_rules, d.E, rs, n);  // exact on the hostname key
       for (int k = 0; rs >= 0 && k < d.K && bit; k++) {
         Slot pod = rs_slot(d, rs, k);
         if (!slot_present(pod)) continue;

@@ -464,6 +464,19 @@ __device__ __forceinline__ void store_class_regs(const KpDev& d, PodCtx& px, con
   if (lane == 0) px.n_hc = sm ? __popc(hm) : -1;
 }
 
+// TopologyNodeFilter.Matches of a filter whose alternatives carry host rules (KpGroup::affinity_policy 3): an alternative
+// matches when the placement's requirement slots are compatible with it and its host rule admits `host`.  A branch of its
+// own, so that topo_record's loop for every other group stays as it was.
+__device__ __forceinline__ bool filter_matches_host_rules(const KpDev& d, const KpGroup& G, const Slot& F, int host, int lane) {
+  for (int a = 0; a < G.filter_n; a++) {
+    const int rs = d.filter_rs[G.filter_off + a];
+    const bool bad = lane < d.K &&
+                     !slot_compatible(key_info(d, lane), F, rs_slot(d, rs, lane), d.key_wellknown[lane], false);
+    if (!__any_sync(FULL, bad) && host_rule_admits(d.host_rules, d.E, rs, host)) return true;
+  }
+  return false;
+}
+
 // Topology.Record (topology.go:197-220) for the committed placement; executed by one warp.
 __device__ __forceinline__ void topo_record(const KpDev& d, const PodCtx& px, const Slot& F, int taintset, int host,
                                             bool allow_undef, int lane) {
@@ -489,6 +502,8 @@ __device__ __forceinline__ void topo_record(const KpDev& d, const PodCtx& px, co
           }
         }
         counts = any_alt;
+      } else if (G.affinity_policy == 3) {
+        counts = filter_matches_host_rules(d, G, F, host, lane);
       }
       if (counts && G.taint_policy == 1) {
         counts = tolerated(d, G.tolset, taintset);

@@ -197,6 +197,88 @@ static int validate_problem(const kp_problem* p, std::string& err) {
   return KP_OK;
 }
 
+// ---- host rules: requirements on kubernetes.io/hostname ----
+// Per requirement set, its hostname entries folded with Requirements.Add (requirement.go Intersection) into
+// {complement, sorted value ids}, on value sets of any size: the key keeps its exemption from the 64 values of a slot.
+// Slot rows never carry the key; the rule is an admission test of candidates instead (host_rule_admits, kp_slot.hpp).
+// Distinct rules share one record of KpDev::host_rules.
+static int build_host_rules(const kp_problem* p, HostTables& h, bool serve, std::string& err) {
+  const int S = p->n_reqsets, E = h.E, EW = (E + 31) / 32;
+  h.rs_rule.assign(std::max(S, 1), -1);
+  h.host_rules.assign(std::max(S, 1), -1);
+  h.rule_exists.clear();
+  h.n_rules = 0;
+  if (h.hostname_key < 0) return KP_OK;
+  std::map<std::pair<bool, std::vector<int32_t>>, int> distinct;
+  std::vector<int32_t> rule_off;
+  std::multimap<int32_t, int> nodes_of;  // hostname value id -> existing nodes carrying it
+  for (int n = 0; n < E; n++) nodes_of.emplace(p->node_hostname[n], n);
+  for (int s = 0; s < S; s++) {
+    bool any = false, comp = false;
+    std::vector<int32_t> vals;
+    for (int e = p->reqset_off[s]; e < p->reqset_off[s + 1]; e++) {
+      if (p->req_key[e] != h.hostname_key) continue;
+      if (!serve) return err = "requirements on kubernetes.io/hostname are not supported by this solver", KP_ERR_UNSUPPORTED;
+      const uint8_t f = p->req_flags[e];
+      if (f & (KP_REQ_HAS_GTE | KP_REQ_HAS_LTE))
+        return err = "Gt / Lt on kubernetes.io/hostname is not supported", KP_ERR_UNSUPPORTED;
+      if (f & KP_REQ_HAS_MINVALUES) return err = "minValues on kubernetes.io/hostname is not supported", KP_ERR_UNSUPPORTED;
+      std::vector<int32_t> in(p->req_vals + p->req_val_off[e], p->req_vals + p->req_val_off[e + 1]), out;
+      std::sort(in.begin(), in.end());
+      in.erase(std::unique(in.begin(), in.end()), in.end());
+      const bool ic = (f & KP_REQ_COMPLEMENT) != 0;
+      if (!any) {
+        any = true;
+        comp = ic;
+        vals = std::move(in);
+        continue;
+      }
+      if (!comp && !ic)
+        std::set_intersection(vals.begin(), vals.end(), in.begin(), in.end(), std::back_inserter(out));
+      else if (!comp)
+        std::set_difference(vals.begin(), vals.end(), in.begin(), in.end(), std::back_inserter(out));
+      else if (!ic)
+        std::set_difference(in.begin(), in.end(), vals.begin(), vals.end(), std::back_inserter(out));
+      else
+        std::set_union(vals.begin(), vals.end(), in.begin(), in.end(), std::back_inserter(out));
+      comp = comp && ic;
+      vals = std::move(out);
+    }
+    if (!any) continue;
+    auto it = distinct.emplace(std::make_pair(comp, vals), h.n_rules).first;
+    if (it->second == h.n_rules) {  // a new rule: {admits NodeClaims, admitted existing nodes}
+      h.n_rules++;
+      h.rule_exists.push_back(comp && vals.empty());
+      rule_off.push_back((int32_t)h.host_rules.size());
+      h.host_rules.push_back(comp ? 1 : 0);
+      h.host_rules.resize(h.host_rules.size() + EW, 0);
+      int32_t* words = h.host_rules.data() + rule_off.back() + 1;
+      if (comp)  // every node, then flip the ones the rule names
+        for (int n = 0; n < E; n++) words[n >> 5] |= (int32_t)(1u << (n & 31));
+      for (int32_t v : vals)
+        for (auto r = nodes_of.equal_range(v); r.first != r.second; ++r.first)
+          words[r.first->second >> 5] ^= (int32_t)(1u << (r.first->second & 31));
+    }
+    h.rs_rule[s] = it->second;
+    h.host_rules[s] = rule_off[it->second];
+  }
+  // A NodePool, instance type or offering on the hostname key would have to be matched against the placeholders
+  for (int n = 0; n < p->n_templates; n++)
+    if (h.rs_rule[p->tmpl_reqset[n]] >= 0)
+      return err = "requirements on kubernetes.io/hostname in a NodePool template are not supported", KP_ERR_UNSUPPORTED;
+  for (int t = 0; t < p->n_its; t++) {
+    if (h.rs_rule[p->it_reqset[t]] >= 0)
+      return err = "requirements on kubernetes.io/hostname on an instance type are not supported", KP_ERR_UNSUPPORTED;
+    for (int o = p->it_off_off[t]; o < p->it_off_off[t + 1]; o++)
+      if (h.rs_rule[p->off_reqset[o]] >= 0)
+        return err = "requirements on kubernetes.io/hostname on an offering are not supported", KP_ERR_UNSUPPORTED;
+  }
+  for (int n = 0; n < E; n++)
+    if (h.rs_rule[p->node_reqset[n]] >= 0)
+      return err = "invalid problem: node_reqset carries kubernetes.io/hostname (a node's hostname is node_hostname)", KP_ERR_INVALID;
+  return KP_OK;
+}
+
 // ---- which shortcuts each class may take (ClassPlan), from the finished tables ----
 static void plan_classes(const Ctx& c, HostTables& h) {
   const int K = h.K, N = h.N, X = h.X, X1 = std::max(X, 1);
@@ -227,13 +309,21 @@ static void plan_classes(const Ctx& c, HostTables& h) {
     if (ac && bc) return (bm & ~am) == 0;
     return false;
   };
+  // every candidate the host rule of rs_a admits (existing nodes and NodeClaims) is one the rule of rs_b admits
+  auto host_implied = [&](int rs_a, int rs_b) {
+    if (h.rs_rule[rs_b] < 0) return true;
+    if (h.admits_claims(rs_a) && !h.admits_claims(rs_b)) return false;
+    for (int n = 0; n < h.E; n++)
+      if (h.admits_node(rs_a, n) && !h.admits_node(rs_b, n)) return false;
+    return true;
+  };
   // TopologyNodeFilter.Matches (topologynodefilter.go:68-97) holds for every claim whose requirements the class's
   // own requirement set leaves unchanged: some alternative is empty, or constrains only keys the class constrains
-  // at least as tightly
+  // at least as tightly (on the hostname key: admits every candidate the class's host rule admits)
   auto filter_implied = [&](int x, const KpGroup& G) {
     for (int a = 0; a < G.filter_n; a++) {
       const int rs = h.filter_rs[G.filter_off + a];
-      bool ok = true;
+      bool ok = host_implied(h.cls_rs[x], rs);
       for (int k = 0; k < K && ok; k++) {
         if (!(h.rs_flags[(size_t)rs * K + k] & SF_PRESENT)) continue;
         ok = (h.rs_flags[(size_t)h.cls_rs[x] * K + k] & SF_PRESENT) && slot_subset(h.cls_rs[x], rs, k);
@@ -304,11 +394,15 @@ static void plan_classes(const Ctx& c, HostTables& h) {
         has_tk = true;
       else if (G.key != h.hostname_key)
         fp = false;
-      if (fp && !G.inverse && G.affinity_policy == 1 && G.filter_n > 0 && !filter_implied(x, G)) fp = false;
+      if (fp && !G.inverse && (G.affinity_policy & 1) && G.filter_n > 0 && !filter_implied(x, G)) fp = false;
     }
     pl.fp[x] = fp;
     pl.has_tk[x] = fp && has_tk;
-    for (int n = 0; n < std::min(N, 64); n++) {
+    // a class whose host rule admits no NodeClaim (In / DoesNotExist on the hostname key) tolerates no template, which
+    // skips both NodeClaim stages; a volume-alternative chain only when none of its alternatives admits one
+    bool claims = false;
+    for (int a = x; a >= 0 && !claims; a = h.cls_vol_next[a]) claims = h.admits_claims(h.cls_rs[a]);
+    for (int n = 0; n < std::min(N, 64) && claims; n++) {
       const int ts = h.tmpl_taintset[n];
       if (ts < 0 || h.n_taintsets == 0 || h.tol_ok[(size_t)(h.cls_tolset[x] + 1) * h.n_taintsets + ts]) pl.tok[x] |= 1ull << n;
     }
@@ -341,7 +435,7 @@ static void plan_classes(const Ctx& c, HostTables& h) {
 
 int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
                const std::vector<std::pair<int, int>>& extra_bound, const std::vector<int32_t>& pending_classes,
-               HostTables& h, std::string& err) {
+               HostTables& h, std::string& err, bool host_rules) {
   {
     int rc = validate_problem(p, err);
     if (rc != KP_OK) return rc;
@@ -422,7 +516,7 @@ int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
     for (int e = p->reqset_off[s]; e < p->reqset_off[s + 1]; e++) {
       int k = p->req_key[e];
       uint8_t f = p->req_flags[e];
-      if (k == h.hostname_key) return err = "requirements on kubernetes.io/hostname are not supported yet", KP_ERR_UNSUPPORTED;
+      if (k == h.hostname_key) continue;  // the set's host rule (build_host_rules)
       Slot in;
       in.f = SF_PRESENT | ((f & KP_REQ_COMPLEMENT) ? SF_COMPLEMENT : 0) | ((f & KP_REQ_HAS_GTE) ? SF_HAS_GTE : 0) |
              ((f & KP_REQ_HAS_LTE) ? SF_HAS_LTE : 0);
@@ -440,6 +534,10 @@ int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
       h.rs_lte[i] = out.lte;
       h.rs_keys[s] |= 1u << k;
     }
+  }
+  {
+    const int rc = build_host_rules(p, h, host_rules, err);
+    if (rc != KP_OK) return rc;
   }
   // ---- taints ----
   h.n_taintsets = p->n_taintsets;
@@ -743,18 +841,19 @@ int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
     size_t i = (size_t)node * K + k;
     return Slot{h.node_sflags[i], h.node_smask[i], h.node_sgte[i], h.node_slte[i]};
   };
-  auto filter_matches = [&](const HGroup& g, int taintset, auto slot_of) {
+  auto filter_matches = [&](const HGroup& g, int node) {
     bool aff = true;
     if (g.g.affinity_policy == 1 && !g.filter.empty()) {
       aff = false;
       for (int rs : g.filter)
-        if (c.rows_compatible(slot_of, [&](int k) { return c.rs_slot(rs, k); }, false)) {
+        if (h.admits_node(rs, node) &&
+            c.rows_compatible([&](int k) { return node_slot(node, k); }, [&](int k) { return c.rs_slot(rs, k); }, false)) {
           aff = true;
           break;
         }
     }
     bool tnt = true;
-    if (g.g.taint_policy == 1) tnt = c.tolerates(taintset, g.g.tolset);
+    if (g.g.taint_policy == 1) tnt = c.tolerates(p->node_taintset[node], g.g.tolset);
     return aff && tnt;
   };
   auto make_group = [&](int cls, int ci, bool inv) {
@@ -806,6 +905,7 @@ int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
       s.append((const char*)&h.rs_mask[(size_t)r * K], K * 8);
       s.append((const char*)&h.rs_gte[(size_t)r * K], K * 8);
       s.append((const char*)&h.rs_lte[(size_t)r * K], K * 8);
+      s.append((const char*)&h.rs_rule[r], 4);  // distinct rules have distinct ids
       rs.insert(s);
     }
     for (auto& s : rs) o << s << "#";
@@ -930,7 +1030,7 @@ int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
         // countDomains (topology.go:328-426)
         for (int n = 0; n < E; n++) {
           if (!node_active[n]) continue;
-          if (!filter_matches(g, p->node_taintset[n], [&](int k) { return node_slot(n, k); })) continue;
+          if (!filter_matches(g, n)) continue;
           int d;
           if (node_domain(n, g.g.key, &d)) group_register(g, d);
         }
@@ -940,7 +1040,7 @@ int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
           if (g.selector >= 0 && !c.selector_matches(g.selector, p->class_labelset[bc])) continue;
           int d;
           if (!node_domain(node, g.g.key, &d)) continue;
-          if (!filter_matches(g, p->node_taintset[node], [&](int k) { return node_slot(node, k); })) continue;
+          if (!filter_matches(g, node)) continue;
           group_record(g, d);
         }
         g.lazy = pi >= n_direct;
@@ -992,7 +1092,10 @@ int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
     g.g.dom_off = gi * 64;
     g.g.filter_off = (int)h.filter_rs.size();
     g.g.filter_n = (int)g.filter.size();
-    for (int r : g.filter) h.filter_rs.push_back(r);
+    for (int r : g.filter) {
+      h.filter_rs.push_back(r);
+      if (g.g.affinity_policy == 1 && h.rs_rule[r] >= 0) g.g.affinity_policy = 3;  // the record test reads the rules
+    }
     if (g.g.key == h.hostname_key) {
       g.g.host_row = GH++;
       h.g_ndomains[gi] = (int)g.host_reg.size();
@@ -1090,6 +1193,19 @@ int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
   if (h.cls_match.empty()) h.cls_match.push_back(0);
   if (h.cls_rec.empty()) h.cls_rec.push_back(0);
   (void)host_to_node;
+  // Hostname-key pod affinity bootstraps on "is some domain the pod may take populated" (anyCompatiblePodDomain,
+  // topologygroup.go:326,383-390); the solver keeps one "any domain populated" flag per group (KpDev::g_anypop), which
+  // answers it only for a pod that may take every domain
+  for (int x = 0; x < X; x++) {
+    bool restricted = false;
+    for (int rs : {h.cls_rs[x], h.cls_strict_rs[x]}) restricted |= h.rs_rule[rs] >= 0 && !h.rule_exists[h.rs_rule[rs]];
+    for (int i = h.cls_match_off[x]; i < h.cls_match_off[x + 1] && restricted; i++) {
+      const KpGroup& G = h.groups[h.cls_match[i] & 0x3fffffff];
+      if (G.key == h.hostname_key && G.type == KP_TOPO_AFFINITY)
+        return err = "a requirement on kubernetes.io/hostname together with pod affinity on kubernetes.io/hostname is not supported",
+               KP_ERR_UNSUPPORTED;
+    }
+  }
   plan_classes(c, h);
   return KP_OK;
 }

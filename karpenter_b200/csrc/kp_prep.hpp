@@ -102,13 +102,21 @@ struct HostTables {
   std::vector<uint64_t> node_smask;
   std::vector<int64_t> node_sgte, node_slte;
   std::vector<int32_t> group_out_order;  // result order: regular groups (creation order) then inverse groups
+  // host rules: [n_reqsets] distinct rule of each requirement set (-1: none), and KpDev::host_rules
+  int n_rules = 0;
+  std::vector<int32_t> rs_rule, host_rules;
+  std::vector<uint8_t> rule_exists;  // [n_rules] the rule is Exists (NotIn{})
+  bool admits_node(int rs, int node) const { return host_rule_admits(host_rules.data(), E, rs, node); }
+  bool admits_claims(int rs) const { return host_rule_admits(host_rules.data(), E, rs, E); }
   ClassPlan plan;
 };
 
-// active: which nodes take part as existing nodes; extra_bound: additional (class,node) pods counted by the topology
+// active: which nodes take part as existing nodes; extra_bound: additional (class,node) pods counted by the topology.
+// host_rules: the caller's solver applies host rules (HostTables::host_rules); any other caller gets KP_ERR_UNSUPPORTED
+// for a requirement on kubernetes.io/hostname instead of tables it would read without them.
 int kp_prepare(const kp_problem* p, const std::vector<uint8_t>& node_active,
                const std::vector<std::pair<int, int>>& extra_bound, const std::vector<int32_t>& pending_classes,
-               HostTables& h, std::string& err);
+               HostTables& h, std::string& err, bool host_rules = false);
 
 // Price lists of offerings: per list, a range [off[i], off[i + 1]) of (price, distinct offering set) entries.  `set` and
 // `price` are never empty, so each uploads as a table of at least one element.

@@ -197,3 +197,13 @@ KP_HD Slot slot_add_nb(const Slot& existing, const Slot& incoming) {
     o.m = incoming.m & existing.m;
   return o;
 }
+
+// The host rule of requirement set rs (KpDev::host_rules) on hostname domain `host`: an existing node (host < E) is
+// admitted iff its hostname satisfies the rule, a NodeClaim iff the rule is a complement (NotIn / Exists).  Every
+// NodeClaim carries hostname In{placeholder} that no pod can name (nodeclaim.go:92-96), every existing node hostname
+// In{its hostname} (existingnode.go:62), so a rule never changes a candidate's requirements, only admits or rejects it.
+KP_HD bool host_rule_admits(const int32_t* host_rules, int E, int rs, int host) {
+  const int o = host_rules[rs];
+  if (o < 0) return true;
+  return host < E ? (((uint32_t)host_rules[o + 1 + (host >> 5)] >> (host & 31)) & 1u) != 0 : host_rules[o] != 0;
+}

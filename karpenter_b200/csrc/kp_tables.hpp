@@ -56,7 +56,8 @@ struct KpGroup {
   int32_t inverse;
   int32_t dom_off;      // offset into dom_cnt (non-hostname groups); hostname groups: row in host_cnt
   int32_t filter_off, filter_n;   // TopologyNodeFilter.Requirements alternatives (reqset ids)
-  int32_t taint_policy, affinity_policy;  // 0 ignore 1 honor 2 unset
+  int32_t taint_policy;
+  int32_t affinity_policy;  // 0 ignore 1 honor 2 unset; 3 honor, and some filter alternative carries a host rule (bit 0: honor)
   int32_t tolset;
   int32_t host_row;     // row index among hostname groups, -1 otherwise
 };
@@ -96,6 +97,7 @@ struct KpDev {
   const uint64_t* offset_bits;    // [D*ITW] types with an AVAILABLE offering of that set
   int tab_bytes;                  // shared-memory bytes of the staged read-only tables (k_solve); 0 = not staged
   int n_ge, n_itv;                // rows of ge_vals / itv
+  int nodes_res;                  // resource index of "pods" (limits), -1: none
   const int64_t* it_capacity;     // [T*R] (limits)
   // templates
   const int32_t* tmpl_rs;         // [N]
@@ -105,7 +107,10 @@ struct KpDev {
   const int64_t* tmpl_daemon;     // [N*R]
   int64_t* tmpl_remaining;        // [N*R] remainingResources (limits)
   const uint32_t* tmpl_limit_present;  // [N]
-  int nodes_res;
+  // Host rules (kp_prep.cpp build_host_rules): the folded kubernetes.io/hostname requirement of a requirement set, as an
+  // admission test of candidates (host_rule_admits).  [n_reqsets] offset of the set's record, -1: no rule; a record is
+  // {admits NodeClaims, ceil(E/32) words of admitted existing nodes}.
+  const int32_t* host_rules;
   // classes
   const int64_t* cls_req;         // [X*R]
   const int32_t* cls_rs;          // [X]
@@ -239,3 +244,6 @@ struct KpDev {
   unsigned long long rsv_val_of[64];             // value bit (in rsv_id_key) of reservation id i
   long long deadline_ns;          // 0 = none; the solve stops with KP_DEADLINE once this much device time has passed
 };
+// The block is copied to every solver CTA's shared memory, whose plan (kp_api.cu plan_solve) is sized around it: a new
+// field takes a padding word (the int fields fill the holes before pointers) rather than growing it.
+static_assert(sizeof(KpDev) == 1600, "KpDev's size is part of the solver's shared-memory plan");

@@ -1047,9 +1047,15 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
               if (!OVERLAY && lane == 0) I.nfit[(size_t)rv * EW + (node >> 5)] &= ~(1u << (node & 31));  // monotone
               continue;
             }
-            Eval ev = eval_candidate<LEAN>(d, px, false, nb, 0, 0, 0, node, scratch, lane);
-            if (VOL && !ev.ok && px.vol_next >= 0) {  // the other volume-topology alternatives (existingnode.go:98-113)
+            // a volume-topology chain is a candidate on every tolerated node (no signature): an alternative whose host
+            // rule rejects the node is skipped
+            const bool chain = VOL && px.vol_next >= 0;
+            Eval ev{};
+            if (!chain || host_rule_admits(d.host_rules, E, d.cls_rs[Xc], node))
+              ev = eval_candidate<LEAN>(d, px, false, nb, 0, 0, 0, node, scratch, lane);
+            if (chain && !ev.ok) {  // the other volume-topology alternatives (existingnode.go:98-113)
               for (int alt = px.vol_next; alt >= 0 && !ev.ok; alt = next_alt(d, alt)) {
+                if (!host_rule_admits(d.host_rules, E, d.cls_rs[alt], node)) continue;
                 load_alt_slots(d, pxw, alt, lane);
                 ev = eval_candidate<LEAN>(d, px, false, nb, 0, 0, 0, node, scratch, lane);
               }
@@ -1373,7 +1379,10 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
           unsigned long long held = 0, take = 0;
           bool alt_loaded = false;
           for (int alt = -1;;) {
-            ev = eval_candidate<LEAN>(d, px, true, b, bq, bi, bj, E + cc, scratch, lane);
+            // an alternative whose host rule admits no NodeClaim fails without an evaluation
+            ev = Eval{};
+            if (!VOL || host_rule_admits(d.host_rules, E, d.cls_rs[alt < 0 ? Xc : alt], E + cc))
+              ev = eval_candidate<LEAN>(d, px, true, b, bq, bi, bj, E + cc, scratch, lane);
             // Strict minValues (nodeclaim.go:464-475): the surviving types must still span enough distinct values
             if (!LEAN && d.mv_strict && ev.ok && !min_values_ok(d, I.c_tmpl[cc], ev.its, lane)) ev.ok = false;
             if (abit && ev.pod_noop && lane == 0) I.amask[cc] |= abit;
@@ -1532,7 +1541,9 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
       unsigned long long take = 0;
       bool rerr = false, alt_loaded = false;
       for (int alt = -1;;) {
-        ev = eval_candidate<LEAN>(d, px, true, b, bq, tw, -1, E + cnew, scratch, lane);
+        ev = Eval{};
+        if (!VOL || host_rule_admits(d.host_rules, E, d.cls_rs[alt < 0 ? Xc : alt], E + cnew))
+          ev = eval_candidate<LEAN>(d, px, true, b, bq, tw, -1, E + cnew, scratch, lane);
         if (!LEAN && d.mv_strict && ev.ok && !min_values_ok(d, n, ev.its, lane)) ev.ok = false;
         take = 0;
         rerr = false;

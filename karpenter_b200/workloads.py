@@ -274,7 +274,7 @@ def config_c5_shards(n_pods=10_000_000, n_pools=8, n_its=1000, app_replicas=1000
 
 
 def config_c4(n_nodes=10_000, n_pods=200_000, n_candidates=100, max_subset=3, n_its=144, catalog="generic",
-              spot_fraction=0.0, spot_to_spot=False, node_cpus=(8, 16), window=4, slack_pods=20):
+              spot_fraction=0.0, spot_to_spot=False, node_cpus=(8, 16), window=4, slack_pods=20, pin_own=0):
     """C4: a cluster of existing KWOK nodes holding `n_pods` running pods + the removal subsets to evaluate.
 
     Returns (EncodedProblem, ConsolInput-kwargs dict).  BASELINE configs[3]: 10 000 nodes, 200 000 running pods, i.e.
@@ -299,6 +299,9 @@ def config_c4(n_nodes=10_000, n_pods=200_000, n_candidates=100, max_subset=3, n_
     any OS and capacity type, so a replacement NodeClaim can carry more than 600 instance types (the price-ordered
     truncation of scheduler.go:361-379); `spot_fraction` of the nodes run on spot capacity (spot-to-spot rules,
     consolidation.go:236-316).
+
+    `pin_own` > 0: on that many nodes one running pod selects its own node by hostname (every tenth candidate, then
+    nodes evenly spread over the rest), so removing such a node leaves that pod nowhere to go.
     """
     from .model import quantity_units
     b = ProblemBuilder()
@@ -401,13 +404,20 @@ def config_c4(n_nodes=10_000, n_pods=200_000, n_candidates=100, max_subset=3, n_
     order = np.argsort(pod_node, kind="stable")
     rows_cls = table[ci, mi][order]
     rows_node = pod_node[order]
-    b.set_pod_arrays(rows_cls, np.zeros(len(rows_cls), np.int64), dp[order, 2], dp[order, 3])
-    enc = b.build()
     counts = np.bincount(rows_node, minlength=n_nodes)
     node_pod_off = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
     # candidates: non-empty nodes sorted by disruption cost (== pod count), ties by index (stable canon)
     nonempty = np.nonzero(counts > 0)[0]
     cand = nonempty[np.argsort(counts[nonempty], kind="stable")][:n_candidates]
+    if pin_own > 0:
+        rest = np.setdiff1d(nonempty, cand)
+        pick = list(cand[::10]) + list(rest[::max(1, len(rest) // pin_own)])
+        for n in pick[:pin_own]:
+            i = node_pod_off[n]  # the node's first pod row
+            rows_cls[i] = b.pod_class(Pod(requests=_requests(ci[order][i], mi[order][i]),
+                                          node_selector={HOSTNAME_LABEL: f"node-{n:05d}"}))
+    b.set_pod_arrays(rows_cls, np.zeros(len(rows_cls), np.int64), dp[order, 2], dp[order, 3])
+    enc = b.build()
     subsets: List[Tuple[int, ...]] = []
     k = len(cand)
     for i in range(k):
@@ -433,10 +443,11 @@ def config_c4(n_nodes=10_000, n_pods=200_000, n_candidates=100, max_subset=3, n_
     return enc, consol
 
 
-def config_existing(n_nodes=200, n_pods=3000, n_its=50, fill=0.6, limits=None) -> EncodedProblem:
+def config_existing(n_nodes=200, n_pods=3000, n_its=50, fill=0.6, limits=None, pin_in=0.0, pin_not_in=0.0) -> EncodedProblem:
     """Provisioning against a live cluster: `n_nodes` existing KWOK nodes (zone / arch / capacity-type labels, a third
     of them tainted, `fill` of their allocatable already used) + pending pods with zone / arch selectors and
-    tolerations.  Exercises addToExistingNode (scheduler.go:520-555) before the NodeClaim stages."""
+    tolerations.  Exercises addToExistingNode (scheduler.go:520-555) before the NodeClaim stages.  `pin_in` of the pods
+    select one of the first 500 nodes by hostname, `pin_not_in` keep off three nodes (NotIn on the hostname)."""
     from .model import quantity_units
     b = ProblemBuilder()
     its = kwok.generic_instance_types()[:n_its]
@@ -484,6 +495,24 @@ def config_existing(n_nodes=200, n_pods=3000, n_its=50, fill=0.6, limits=None) -
                         tols = [Toleration("bench/dedicated", "Exists", "", "")] if k else []
                         table[c, m, z + 1, a + 1, k] = b.pod_class(
                             Pod(requests=_requests(c, m), node_selector=sel, tolerations=tols))
-    b.set_pod_arrays(table[ci, mi, zsel + 1, asel + 1, tol], np.zeros(n_pods, np.int64), d[:, 7],
-                     splitmix64(SEED + 22, np.arange(n_pods, dtype=np.uint64)))
+    cls = table[ci, mi, zsel + 1, asel + 1, tol]
+    if pin_in or pin_not_in:
+        h = draws(n_pods, 4, SEED + 23)
+        u = (h[:, 0] % np.uint64(10_000)).astype(int)
+        for i in np.flatnonzero(u < int((pin_in + pin_not_in) * 10_000)):
+            sel = {}
+            if zsel[i] >= 0:
+                sel[ZONE_LABEL] = kwok.KWOK_ZONES[zsel[i]]
+            if asel[i] >= 0:
+                sel[ARCH_LABEL] = archs[asel[i]]
+            aff = []
+            if u[i] < int(pin_in * 10_000):
+                sel[HOSTNAME_LABEL] = f"node-{int(h[i, 1] % np.uint64(min(500, n_nodes))):05d}"
+            else:
+                hosts = tuple(f"node-{int(h[i, k] % np.uint64(n_nodes)):05d}" for k in (1, 2, 3))
+                aff = [[NodeSelectorRequirement(HOSTNAME_LABEL, "NotIn", hosts)]]
+            tols = [Toleration("bench/dedicated", "Exists", "", "")] if tol[i] else []
+            cls[i] = b.pod_class(Pod(requests=_requests(ci[i], mi[i]), node_selector=sel, node_affinity_required=aff,
+                                     tolerations=tols))
+    b.set_pod_arrays(cls, np.zeros(n_pods, np.int64), d[:, 7], splitmix64(SEED + 22, np.arange(n_pods, dtype=np.uint64)))
     return b.build()
