@@ -251,34 +251,15 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CQ, in
     I.pmask = d.pmask;
     I.amask = d.amask;
     I.tmpl_remaining = d.tmpl_remaining;
-    I.node_rem = d.node_rem;
-    I.node_rem_present = d.node_rem_present;
-    I.node_sflags = d.node_sflags;
-    I.node_smask = d.node_smask;
-    I.node_sgte = d.node_sgte;
-    I.node_slte = d.node_slte;
-    I.node_npods = d.node_npods;
-    I.nfit = d.nfit;
-    I.nstat = d.nstat;
-    I.nactive = d.nactive;
-    I.nfit_sum = d.nfit_sum;
-    I.nstat_sum = d.nstat_sum;
     I.n_removed = 0;
     I.removed = nullptr;
     I.ov_cap = 0;
     I.n_ov = 0;
     I.CS = 0;
-    I.g_order = d.order;
-    I.g_cnt_at = d.cnt_at;
-    I.g_c_tmpl = d.c_tmpl;
-    I.g_pmask = d.pmask;
-    I.g_amask = d.amask;
     I.c_dom = d.c_dom;
-    I.g_c_dom = d.c_dom;
     I.rsv_cap = d.rsv_cap;
     I.c_rsv = d.c_rsv;
     I.c_ports = d.c_ports;
-    I.node_ports = d.node_ports;
     I.ov_ports = nullptr;
     I.CQ = 0;
     I.CR = 0;
@@ -314,7 +295,7 @@ __device__ __forceinline__ void wsolve_cta(const KpDev& d_in, int CS, int CQ, in
     stager_run<COHORT>(d, I, &sh.ring, lane);
     return;
   }
-  wsolve_run<false, true, LEAN, COHORT, VOL>(d, I, sh.ring.slot[0], sh.scratch, lane, &sh.ring);
+  wsolve_run<false, LEAN, COHORT, VOL>(d, I, sh.ring.slot[0], sh.scratch, lane, &sh.ring);
   const int nC = I.n_claims;
   claim_rows_flush(d, I, nC, lane);
   if (ntk > 0) {  // before k_scatter_counts, the counter all-reduce and the download read them
@@ -836,28 +817,14 @@ __global__ void __launch_bounds__(CONSOL_WARPS * 32, CONSOL_MIN_CTAS) k_consolid
     I.pmask = w.pmask;
     I.amask = w.amask;
     I.tmpl_remaining = w.tmpl_remaining;
-    I.node_rem = d.node_rem;  // shared base, read-only here
-    I.node_rem_present = d.node_rem_present;
-    I.node_sflags = d.node_sflags;
-    I.node_smask = d.node_smask;
-    I.node_sgte = d.node_sgte;
-    I.node_slte = d.node_slte;
-    I.node_npods = nullptr;
-    I.nfit = d.nfit;
-    I.nstat = d.nstat;
-    I.nactive = d.nactive;
-    I.nfit_sum = d.nfit_sum;
-    I.nstat_sum = d.nstat_sum;
     I.CS = 0;
     I.CQ = 0;
     I.CR = 0;
     I.c_dom = nullptr;  // candidate sets with topology take the batch path (k_wsolve_batch)
-    I.g_c_dom = nullptr;
     I.rsv_cap = w.rsv_cap;
     I.c_rsv = w.c_rsv;
     I.c_ports = w.c_ports;
     I.ov_ports = w.ov_ports;
-    I.node_ports = d.node_ports;  // shared base, read-only here
     I.ov_cap = capq;
     I.ov_node = w.ov_node;
     I.ov_rem = w.ov_rem;
@@ -950,7 +917,7 @@ __global__ void __launch_bounds__(CONSOL_WARPS * 32, CONSOL_MIN_CTAS) k_consolid
       I.tmpl_remaining[i] = rem;
     }
     __syncwarp();
-    wsolve_run<true, false, LEAN>(d, I, W.ctx, W.scratch, lane);
+    wsolve_run<true, LEAN>(d, I, W.ctx, W.scratch, lane);
     if (I.status != KP_OK) {
       if (lane == 0) *q.status = I.status;
       break;

@@ -80,32 +80,24 @@ struct WInst {
   // (the claim's value sets only shrink, so they stay inside the pod's), which reduces CanAdd for such a pair to the
   // resource test.
   unsigned long long* amask;
-  unsigned long long* g_amask;
   // c_dom[c]: the value claim c's slot on the topology key is pinned to, 0xff when it is not a single In value (null: the
   // instance does not use the domain fast path)
-  uint8_t *c_dom, *g_c_dom;
+  // (The solver loads this block from shared memory in 16-byte pairs, and the schedule of its chain moves with that
+  // pairing: with amask / c_dom sharing a pair, C3 took 1.5 % longer.  The alignas below keep amask, c_dom and c_ports
+  // each in a pair of their own and every later field at its offset modulo 16.)
+  alignas(16) uint8_t* c_dom;
   // ReservationManager state of the instance (reservationmanager.go:28-110): remaining capacity per reservation id and
   // the ids each NodeClaim holds (null / unused when the problem has no reserved offerings)
-  int32_t* rsv_cap;
+  alignas(16) int32_t* rsv_cap;
   unsigned long long* c_rsv;
-  // host ports in use per NodeClaim / per existing node (direct mode) / per overlay entry (consolidation)
-  unsigned long long *c_ports, *node_ports, *ov_ports;
+  // host ports in use per NodeClaim / per overlay entry (consolidation)
+  unsigned long long* c_ports;
+  alignas(16) unsigned long long* ov_ports;
   // While the claim order, template ids and failure masks fit, they live in shared memory (CS = claims the shared
-  // copies can hold, 0 = not in use); the moment a claim id reaches CS everything migrates to the global arrays below.
+  // copies can hold, 0 = not in use); the moment a claim id reaches CS everything migrates to the KpDev's global arrays.
   int CS;
-  int32_t *g_order, *g_cnt_at, *g_c_tmpl;
-  ulonglong2* g_pmask;
   int64_t* tmpl_remaining;  // [N*R]
-  // existing nodes
-  int64_t* node_rem;
-  uint32_t* node_rem_present;
-  uint8_t* node_sflags;
-  uint64_t* node_smask;
-  int64_t *node_sgte, *node_slte;
-  int32_t* node_npods;      // direct mode only
-  uint32_t *nfit, *nstat;
-  const uint32_t* nactive;
-  const uint32_t *nfit_sum, *nstat_sum;  // one bit per bitmap word: skip 1024-node chunks nothing can match in
+  // existing nodes: the KpDev's node tables, plus (consolidation) the nodes taken out and a private overlay
   int n_removed;
   const int32_t* removed;   // overlay mode: nodes taken out of the cluster (the consolidation candidates)
   // overlay (consolidation): entry i shadows node ov_node[i]
@@ -474,24 +466,25 @@ __device__ __forceinline__ bool fp_fit(const KpDev& d, const WInst& I, const Pod
   return ok;
 }
 
-// shared -> global migration of the small per-claim arrays (see WInst::CS); executed once, by the whole warp
+// shared -> global migration of the small per-claim arrays (see WInst::CS) into the KpDev's arrays; executed once, by the
+// whole warp.  Only the batch kernel migrates: k_consolidate runs with CS = 0.
 __device__ __forceinline__ void migrate_small(const KpDev& d, WInst& I, int nC, int lane) {
   for (int i = lane; i < nC; i += 32) {
-    I.g_order[i] = I.order[i];
-    I.g_cnt_at[i] = I.cnt_at[i];
-    I.g_c_tmpl[i] = I.c_tmpl[i];
-    I.g_pmask[i] = I.pmask[i];
-    I.g_amask[i] = I.amask[i];
-    if (I.c_dom) I.g_c_dom[i] = I.c_dom[i];
+    d.order[i] = I.order[i];
+    d.cnt_at[i] = I.cnt_at[i];
+    d.c_tmpl[i] = I.c_tmpl[i];
+    d.pmask[i] = I.pmask[i];
+    d.amask[i] = I.amask[i];
+    if (I.c_dom) d.c_dom[i] = I.c_dom[i];
   }
   __syncwarp();
   if (lane == 0) {
-    I.order = I.g_order;
-    I.cnt_at = I.g_cnt_at;
-    I.c_tmpl = I.g_c_tmpl;
-    I.pmask = I.g_pmask;
-    I.amask = I.g_amask;
-    if (I.c_dom) I.c_dom = I.g_c_dom;
+    I.order = d.order;
+    I.cnt_at = d.cnt_at;
+    I.c_tmpl = d.c_tmpl;
+    I.pmask = d.pmask;
+    I.amask = d.amask;
+    if (I.c_dom) I.c_dom = d.c_dom;
     I.CS = 0;
   }
   __syncwarp();
@@ -850,15 +843,17 @@ __device__ __forceinline__ void load_alt_slots(const KpDev& d, PodCtx& px, int a
 }
 __device__ __forceinline__ int next_alt(const KpDev& d, int alt) { return d.cls_lane[(size_t)alt * 32 + KP_HDR + 10].hdr; }
 
-// One Scheduler.Solve over the instance's queue.  OVERLAY: existing-node state = shared base + private overlay.
-// STAGED: pods arrive through a StageRing filled by a second warp instead of being staged inline.
+// One Scheduler.Solve over the instance's queue.  Existing-node state is the KpDev's node tables.
+// CONSOL: hosted by a k_consolidate warp: the node tables are a shared read-only base under the instance's private overlay,
+// and pods are staged inline.  Otherwise (k_wsolve_batch) the solve updates the node tables in place and pods arrive
+// through a StageRing filled by a second warp.
 // COHORT: runs of identical pods may commit in one step (cohort_try); instantiated separately because the mere call site
 // costs the ordinary path 7 % (register allocation of a 250-register loop) -- the host picks it when the queue has runs.
 // VOL: some pod has several volume-topology alternatives (kp_problem.class_vol_next): every candidate evaluation walks the
 // pod's chain of alternative requirement rows; compiled into an instantiation of its own for the same reason as COHORT.
 // LEAN: no topology group, Gt / Lt bound, minValues or reservation anywhere in the problem (the host decides): the code for
 // them is not even compiled into that instance, which keeps the serial chain's instruction footprint small.
-template <bool OVERLAY, bool STAGED, bool LEAN = false, bool COHORT = false, bool VOL = false>
+template <bool CONSOL, bool LEAN = false, bool COHORT = false, bool VOL = false>
 __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch, const int lane, StageRing* ring = nullptr) {
   const int K = d.K, R = d.R, ITW = d.ITW, E = d.E, EW = d.EW;
   const int P = I.P;
@@ -879,9 +874,9 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
     alive_tmpl += __any_sync(FULL, w != 0) ? 1 : 0;
   }
   int n_active_nodes = 0;
-  for (int w = lane; w < EW; w += 32) n_active_nodes += __popc(I.nactive[w]);
+  for (int w = lane; w < EW; w += 32) n_active_nodes += __popc(d.nactive[w]);
   for (int o = 16; o; o >>= 1) n_active_nodes += __shfl_xor_sync(FULL, n_active_nodes, o);
-  if (OVERLAY) n_active_nodes -= I.n_removed;
+  if (CONSOL) n_active_nodes -= I.n_removed;
 
   // software pipeline of the class-row staging: `pf` holds the class row of queue index pf_idx (loads issued one
   // iteration ahead), `ids` the (class, pod) of queue index ids_idx (two iterations ahead)
@@ -929,7 +924,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
     const int h = head;
     const int hq1 = hq + 1 >= cap ? hq + 1 - cap : hq + 1, hq2 = hq1 + 1 >= cap ? hq1 + 1 - cap : hq1 + 1;
     int li, X;
-    if (STAGED) {
+    if (!CONSOL) {
       if (lane == 0) ring->consumed = h;  // every slot below h is free again
       while (ring->produced <= h) {
       }
@@ -948,7 +943,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
     if (h >= P && I.last_len[li] == len) break;  // a full cycle without progress
     head = h + 1;
     hq = hq1;
-    if (!STAGED) {
+    if (CONSOL) {
       {
         ClassRegs cur = pf_idx == h ? pf : load_class_regs(d, X, li, lane);
         __syncwarp();
@@ -976,7 +971,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
         ids_idx = h + 2;
       }
     }
-    PodCtx& pxw = STAGED ? ring->slot[h & (KP_RING - 1)] : ctx;
+    PodCtx& pxw = CONSOL ? ctx : ring->slot[h & (KP_RING - 1)];
     int Xc = X;  // class the pod is tried as: X, then its relaxations (trySchedule, scheduler.go:438-469)
   try_pod:
     const PodCtx& px = pxw;
@@ -988,21 +983,21 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
 
     // ================= addToExistingNode (scheduler.go:520-555) =================
     if (E > 0 && px.nsig >= 0) {
-      const uint32_t* fitrow = I.nfit + (size_t)rv * EW;
-      const uint32_t* strow = I.nstat + (size_t)px.nsig * EW;
+      const uint32_t* fitrow = d.nfit + (size_t)rv * EW;
+      const uint32_t* strow = d.nstat + (size_t)px.nsig * EW;
       int seen = 0;
       // chunks of 32 bitmap words (1024 nodes) that can hold a candidate at all, from the word-level summaries: one
       // parallel load for up to 32 chunks (32 768 nodes); clusters beyond that scan every chunk
       unsigned live = 0xffffffffu;
       if (d.ESW <= 32) {
-        const uint32_t sw = lane < d.ESW ? (I.nfit_sum[(size_t)rv * d.ESW + lane] & I.nstat_sum[(size_t)px.nsig * d.ESW + lane]) : 0u;
+        const uint32_t sw = lane < d.ESW ? (d.nfit_sum[(size_t)rv * d.ESW + lane] & d.nstat_sum[(size_t)px.nsig * d.ESW + lane]) : 0u;
         live = __ballot_sync(FULL, sw != 0);
       }
       for (int w0 = 0; w0 < EW && !found; w0 += 32) {
         if (d.ESW <= 32 && !((live >> (w0 >> 5)) & 1u)) continue;
         const int w = w0 + lane;
-        uint32_t bits = w < EW ? (fitrow[w] & strow[w] & I.nactive[w]) : 0u;
-        if (OVERLAY)
+        uint32_t bits = w < EW ? (fitrow[w] & strow[w] & d.nactive[w]) : 0u;
+        if (CONSOL)
           for (int i = 0; i < I.n_removed; i++)
             if ((I.removed[i] >> 5) == w) bits &= ~(1u << (I.removed[i] & 31));
         unsigned has = __ballot_sync(FULL, bits != 0);
@@ -1017,23 +1012,23 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
             seen++;
             // current state of the node
             int oi = -1;
-            if (OVERLAY) oi = ov_find(I, node, lane);
+            if (CONSOL) oi = ov_find(I, node, lane);
             Slot nb = slot_absent();
             int64_t rem = 0;
             uint32_t pr;
-            if (OVERLAY && oi >= 0) {
+            if (CONSOL && oi >= 0) {
               if (lane < K) nb = load_slot(I.ov_sflags, I.ov_smask, I.ov_sgte, I.ov_slte, (size_t)oi * K + lane, (!LEAN && d.has_bounds));
               if (lane < R) rem = I.ov_rem[(size_t)oi * R + lane];
               pr = I.ov_present[oi];
-            } else {
+            } else {  // (CONSOL: the shared base, read-only here)
               if (lane < K)
-                nb = load_slot(I.node_sflags, I.node_smask, I.node_sgte, I.node_slte, (size_t)node * K + lane, (!LEAN && d.has_bounds));
-              if (lane < R) rem = I.node_rem[(size_t)node * R + lane];
-              pr = I.node_rem_present[node];
+                nb = load_slot(d.node_sflags, d.node_smask, d.node_sgte, d.node_slte, (size_t)node * K + lane, (!LEAN && d.has_bounds));
+              if (lane < R) rem = d.node_rem[(size_t)node * R + lane];
+              pr = d.node_rem_present[node];
             }
             // HostPortUsage.Conflicts (existingnode.go:76-82)
             if (!LEAN && px.port_conf) {
-              const unsigned long long used = (OVERLAY && oi >= 0) ? I.ov_ports[oi] : I.node_ports[node];
+              const unsigned long long used = (CONSOL && oi >= 0) ? I.ov_ports[oi] : d.node_ports[node];
               if (used & px.port_conf) continue;
             }
             // resources.Fits(pod requests, remaining) (resources.go:150-163)
@@ -1044,7 +1039,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
               if (px.req[lane] > (present ? rem : 0)) bad = true;
             }
             if (__any_sync(FULL, bad)) {
-              if (!OVERLAY && lane == 0) I.nfit[(size_t)rv * EW + (node >> 5)] &= ~(1u << (node & 31));  // monotone
+              if (!CONSOL && lane == 0) d.nfit[(size_t)rv * EW + (node >> 5)] &= ~(1u << (node & 31));  // monotone
               continue;
             }
             // a volume-topology chain is a candidate on every tolerated node (no signature): an alternative whose host
@@ -1063,7 +1058,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
             }
             if (!ev.ok) continue;
             // ExistingNode.Add (existingnode.go:147-155)
-            if (OVERLAY) {
+            if (CONSOL) {
               const bool oi_new = oi < 0;
               if (oi < 0) {
                 oi = I.n_ov;
@@ -1087,23 +1082,23 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
               }
               if (lane < R) I.ov_rem[(size_t)oi * R + lane] = rem - px.req[lane];
               if (lane == 0) I.ov_present[oi] = pr | ((1u << R) - 1);
-              if (!LEAN && d.n_hostports && lane == 0) I.ov_ports[oi] = (oi_new ? I.node_ports[node] : I.ov_ports[oi]) | px.ports;
+              if (!LEAN && d.n_hostports && lane == 0) I.ov_ports[oi] = (oi_new ? d.node_ports[node] : I.ov_ports[oi]) | px.ports;
               __syncwarp();
             } else {
               if (ev.changed && lane < K) {
                 const size_t i = (size_t)node * K + lane;
-                I.node_sflags[i] = (uint8_t)ev.F.f;
-                I.node_smask[i] = ev.F.m;
+                d.node_sflags[i] = (uint8_t)ev.F.f;
+                d.node_smask[i] = ev.F.m;
                 if ((!LEAN && d.has_bounds)) {
-                  I.node_sgte[i] = ev.F.gte;
-                  I.node_slte[i] = ev.F.lte;
+                  d.node_sgte[i] = ev.F.gte;
+                  d.node_slte[i] = ev.F.lte;
                 }
               }
-              if (lane < R) I.node_rem[(size_t)node * R + lane] = rem - px.req[lane];
+              if (lane < R) d.node_rem[(size_t)node * R + lane] = rem - px.req[lane];
               if (lane == 0) {
-                I.node_rem_present[node] = pr | ((1u << R) - 1);
-                I.node_npods[node]++;
-                if (!LEAN && px.ports) I.node_ports[node] |= px.ports;
+                d.node_rem_present[node] = pr | ((1u << R) - 1);
+                d.node_npods[node]++;
+                if (!LEAN && px.ports) d.node_ports[node] |= px.ports;
               }
             }
             if (lane == 0) {
@@ -1291,7 +1286,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
       // ---- cohorts (cohort_try): a run of identical fast-path pods may commit in one step
       unsigned coh_moved = 0;
       int coh_w0 = 0, coh_gE = 0, coh_extra = 0;
-      bool coh_ok = COHORT && STAGED && !OVERLAY && d.cohort && Xc == X && px.run_n >= 2 && abit != 0 && (fast_ok || dom_fp) &&
+      bool coh_ok = COHORT && !CONSOL && d.cohort && Xc == X && px.run_n >= 2 && abit != 0 && (fast_ok || dom_fp) &&
                     (LEAN || (px.ports == 0 && px.port_conf == 0)) && (fast_ok || !has_tk || n_active_nodes == 0);
       for (int i = sc.hoff; !LEAN && coh_ok && i < sc.hend; i++)
         if ((sc.hc[i].y & 0xff) == KP_TOPO_AFFINITY) coh_ok = false;  // "is any domain populated" changes with every record
@@ -1487,7 +1482,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
         head += coh_extra;
         hq += coh_extra;
         if (hq >= cap) hq -= cap;
-        if (STAGED) {
+        if (!CONSOL) {
           if (lane == 0) ring->skip_to = head;
         }
       }
@@ -1651,7 +1646,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
       }
       tail++;
       tq = tq + 1 >= cap ? tq + 1 - cap : tq + 1;
-      if (STAGED) {
+      if (!CONSOL) {
         __threadfence_block();
         if (lane == 0) ring->tail_pub = tail;
       }
@@ -1662,7 +1657,7 @@ __device__ void wsolve_run(const KpDev& d, WInst& I, PodCtx& ctx, Slot* scratch,
   KP_PROF_LAP(PH_OTHER);
   if (lane == 0) I.prof_total = prof_t - prof_t0;
 #endif
-  if (STAGED) {
+  if (!CONSOL) {
     __syncwarp();
     if (lane == 0) ring->done = 1;
   }

@@ -12,7 +12,7 @@ path, npods = sys.argv[1], float(sys.argv[2])
 srcdir = sys.argv[3] if len(sys.argv) > 3 else os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "karpenter_b200", "csrc")
 MARKS = {
     "kp_wsolve.cuh": [("ov_find", "int ov_find("), ("claim rows", "void claim_load("), ("scan", "struct ScanCtx {"),
-                      ("migrate", "void migrate_small"), ("stager", "struct StageRing {"), ("head", "template <bool OVERLAY"),
+                      ("migrate", "void migrate_small"), ("stager", "struct StageRing {"), ("head", "template <bool CONSOL"),
                       ("pop/stage", "// ---- Queue.Pop"), ("existing", "addToExistingNode (scheduler.go"),
                       ("sort stage", "sort.Slice(newNodeClaims"), ("inflight", "addToInflightNode (scheduler.go"),
                       ("new claim", "addToNewNodeClaim (scheduler.go"), ("requeue/tail", "scheduler.go:415-421: record the error")],

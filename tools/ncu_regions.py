@@ -26,7 +26,7 @@ def find(lines_, txt):
 
 
 marks = [("claim rows", find(src, "void claim_load(")), ("migrate", find(src, "void migrate_small")),
-         ("stager", find(src, "void stager_run")), ("head", find(src, "template <bool OVERLAY")),
+         ("stager", find(src, "void stager_run")), ("head", find(src, "template <bool CONSOL")),
          ("pop/stage", find(src, "// ---- Queue.Pop")), ("existing", find(src, "addToExistingNode (scheduler.go")),
          ("sort stage", find(src, "sort.Slice(newNodeClaims")), ("inflight scan", find(src, "addToInflightNode (scheduler.go")),
          ("inflight eval+commit", find(src, "const int cpos = base + l;")), ("new claim", find(src, "addToNewNodeClaim (scheduler.go")),
