@@ -733,6 +733,9 @@ __global__ void __launch_bounds__(256) k_feasibility(KpDev d, uint64_t* out, int
       uint64_t fw;
       w = filter_its_word(d, scratch, q, lane, &fw) & its;
       __syncwarp();
+      // filterInstanceTypesByRequirements (nodeclaim.go:412-480) keeps nothing when the remaining types fall short of
+      // the template's Strict minValues
+      if (d.mv_strict && !min_values_ok(d, n, w, lane)) w = 0;
       if (any_bad || !tol_ok) w = 0;
       if (lane < d.ITW) out[((size_t)X * d.N + n) * d.ITW + lane] = w;
     }
