@@ -280,7 +280,8 @@ typedef struct kp_problem {
    * existingnode.go:98-113) ----
    * The encoder registers one class per alternative -- the same pod, alternative i added to class_reqset (never to
    * class_strict_reqset: the topology sees the pod's own requirements) -- and chains them: class_vol_next[x] is the class to try
-   * on a candidate that rejected x, -1 at the end.  pod_class names the head of a chain.  NULL: no pod has more than one. */
+   * on a candidate that rejected x, -1 at the end.  pod_class names the head of a chain.  NULL: no pod has more than one.
+   * kp_consolidate serves chains on any pod of the cluster's pod table, extra pods included, as kp_solve does. */
   const int32_t* class_vol_next; /* [n_classes] or NULL */
 } kp_problem;
 

@@ -954,6 +954,26 @@ static const void* solver_kernel(const std::vector<std::unique_ptr<Instance>>& i
               : (cohort ? (const void*)k_wsolve_batch<false, true> : (const void*)k_wsolve_batch<false, false>);
 }
 
+// The consolidation instantiation of a topology-free pass: the volume-alternative one when any class of the cluster has a
+// chain (it is never lean), else LEAN as the host decided
+static const void* consol_kernel(bool lean, bool vol) {
+  if (vol) return (const void*)k_consolidate<false, true>;
+  return lean ? (const void*)k_consolidate<true> : (const void*)k_consolidate<false>;
+}
+
+// name of a solver or consolidation instantiation, for KP_DEBUG
+static const char* kernel_name(const void* fn) {
+  if (fn == (const void*)k_wsolve_batch<true, false>) return "k_wsolve_batch<true, false>";
+  if (fn == (const void*)k_wsolve_batch<true, true>) return "k_wsolve_batch<true, true>";
+  if (fn == (const void*)k_wsolve_batch<false, false>) return "k_wsolve_batch<false, false>";
+  if (fn == (const void*)k_wsolve_batch<false, true>) return "k_wsolve_batch<false, true>";
+  if (fn == (const void*)k_wsolve_batch<false, false, true>) return "k_wsolve_batch<false, false, true>";
+  if (fn == (const void*)k_consolidate<true>) return "k_consolidate<true>";
+  if (fn == (const void*)k_consolidate<false>) return "k_consolidate<false>";
+  if (fn == (const void*)k_consolidate<false, true>) return "k_consolidate<false, true>";
+  return "?";
+}
+
 // Scheduler.Solve of every uploaded instance, a single solve being a batch of one.  In front of the timed window: the
 // dynamic state is restored and the pointer blocks and {CS, CQ, CR} plans are written to the device.  In it: the prep
 // kernels per instance, ONE solver launch (one CTA per instance), truncation and the counter all-reduce.
@@ -1019,7 +1039,7 @@ static int run_solve(kp_handle* h, int64_t deadline_ms, std::vector<int32_t>& st
   cudaEventElapsedTime(&ms, h->ev0, h->ev1);
   h->stats.solve_ms = ms;
   if (h->d_gcnt) cudaEventElapsedTime(&h->allreduce_ms, h->ev3, h->ev1);
-  if (getenv("KP_DEBUG")) fprintf(stderr, "[kp] %d instance(s): step %.3f ms\n", n, ms);
+  if (getenv("KP_DEBUG")) fprintf(stderr, "[kp] %d instance(s), kernel %s: step %.3f ms\n", n, kernel_name(fn), ms);
   for (int b = 0; b < n; b++) CK(cudaMemcpy(&statuses[b], h->insts[b]->dev.status, 4, cudaMemcpyDeviceToHost));
   return KP_OK;
 }
@@ -1470,10 +1490,6 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   Instance& cl = *h->insts[0];
   HostTables& t = cl.host;
   KpDev& d = cl.dev;
-  if (t.has_vol_alts) {
-    h->err = "consolidation with pods that have several volume-topology alternatives is not supported yet";
-    return KP_ERR_UNSUPPORTED;
-  }
   if (t.has_min_values && !t.min_values_strict) {
     // BestEffort lowers minValues per NodeClaim during the simulation (nodeclaim.go:186-191); carrying those per-claim values
     // through RemoveInstanceTypeOptionsByPriceAndMinValues is not built.  Strict (the default policy) is served.
@@ -1752,16 +1768,16 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   KpDev dq = d;  // the cluster's pointer block with k_consolidate's table plan (the upload keeps the solver's)
   dq.tab_bytes = plan_tables(dq, fixed, budget);
   const size_t smem = fixed + dq.tab_bytes + 64;
+  // the solver's `in.lean` predicate (G == 0 here)
+  const bool lean = !t.has_bounds && !t.min_values_strict && t.n_rsv == 0 && d.n_hostports == 0 && !t.has_vol_alts &&
+                    !getenv("KP_NO_LEAN");
+  const void* fn = consol_kernel(lean, t.has_vol_alts);
   if (getenv("KP_DEBUG"))
-    fprintf(stderr, "[kp] consolidate plan: tables %zu B staged of %zu B, %zu B shared\n", (size_t)dq.tab_bytes,
-            kp_tab_bytes(dq), smem);
-  const bool lean = !t.has_bounds && !t.min_values_strict && t.n_rsv == 0 && d.n_hostports == 0 && !getenv("KP_NO_LEAN");  // (G == 0 here)
-  CK(cudaFuncSetAttribute(lean ? k_consolidate<true> : k_consolidate<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    fprintf(stderr, "[kp] consolidate plan: tables %zu B staged of %zu B, %zu B shared, kernel %s\n", (size_t)dq.tab_bytes,
+            kp_tab_bytes(dq), smem, kernel_name(fn));
+  CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int per_sm = 1;
-  if (lean)
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_consolidate<true>, CONSOL_WARPS * 32, smem);
-  else
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_consolidate<false>, CONSOL_WARPS * 32, smem);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, CONSOL_WARPS * 32, smem);
   per_sm = std::max(per_sm, 1);
   int grid = std::min(h->n_sm * per_sm, std::max(1, (S + CONSOL_WARPS - 1) / CONSOL_WARPS));
   const size_t slots = (size_t)grid * CONSOL_WARPS;
@@ -1793,10 +1809,8 @@ static int kp_consolidate_impl(kp_handle* h, const kp_problem* p, const kp_conso
   rc = launch_node_cand(h, cl);
   if (rc != KP_OK) return rc;
   if (S > 0) {
-    if (lean)
-      k_consolidate<true><<<grid, CONSOL_WARPS * 32, smem, h->stream>>>(dq, q);
-    else
-      k_consolidate<false><<<grid, CONSOL_WARPS * 32, smem, h->stream>>>(dq, q);
+    void* args[] = {(void*)&dq, (void*)&q};
+    CK(cudaLaunchKernel(fn, dim3(grid), dim3(CONSOL_WARPS * 32), args, smem, h->stream));
     h->stats.kernel_launches++;
   }
   CK(cudaEventRecord(h->ev1, h->stream));

@@ -782,7 +782,9 @@ struct ConsolShared {
 #ifndef CONSOL_MIN_CTAS
 #define CONSOL_MIN_CTAS 2
 #endif
-template <bool LEAN>
+// VOL: some pod of the cluster has several volume-topology alternatives (kp_problem.class_vol_next); the host launches that
+// instantiation only then, so the other two compile to what they did before it existed.
+template <bool LEAN, bool VOL = false>
 __global__ void __launch_bounds__(CONSOL_WARPS * 32, CONSOL_MIN_CTAS) k_consolidate(const __grid_constant__ KpDev d_in,
                                                                     const __grid_constant__ KpConsol q) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -917,7 +919,7 @@ __global__ void __launch_bounds__(CONSOL_WARPS * 32, CONSOL_MIN_CTAS) k_consolid
       I.tmpl_remaining[i] = rem;
     }
     __syncwarp();
-    wsolve_run<true, LEAN>(d, I, W.ctx, W.scratch, lane);
+    wsolve_run<true, LEAN, false, VOL>(d, I, W.ctx, W.scratch, lane);
     if (I.status != KP_OK) {
       if (lane == 0) *q.status = I.status;
       break;

@@ -274,7 +274,7 @@ def config_c5_shards(n_pods=10_000_000, n_pools=8, n_its=1000, app_replicas=1000
 
 
 def config_c4(n_nodes=10_000, n_pods=200_000, n_candidates=100, max_subset=3, n_its=144, catalog="generic",
-              spot_fraction=0.0, spot_to_spot=False, node_cpus=(8, 16), window=4, slack_pods=20, pin_own=0):
+              spot_fraction=0.0, spot_to_spot=False, node_cpus=(8, 16), window=4, slack_pods=20, pin_own=0, vol_alts=0):
     """C4: a cluster of existing KWOK nodes holding `n_pods` running pods + the removal subsets to evaluate.
 
     Returns (EncodedProblem, ConsolInput-kwargs dict).  BASELINE configs[3]: 10 000 nodes, 200 000 running pods, i.e.
@@ -302,6 +302,12 @@ def config_c4(n_nodes=10_000, n_pods=200_000, n_candidates=100, max_subset=3, n_
 
     `pin_own` > 0: on that many nodes one running pod selects its own node by hostname (every tenth candidate, then
     nodes evenly spread over the rest), so removing such a node leaves that pod nowhere to go.
+
+    `vol_alts` > 0: on that many nodes (picked the same way) the last running pod has two volume-topology alternatives,
+    each a zone (a StorageClass whose allowedTopologies lists two zones, volumetopology.go:44-125).  On every other such
+    node the first alternative is the node's own zone and the second the next zone; on the rest the first is a zone no
+    node and no offering has, and the second the node's own zone, which is then what places the pod and what pins a
+    replacement NodeClaim.
     """
     from .model import quantity_units
     b = ProblemBuilder()
@@ -416,6 +422,16 @@ def config_c4(n_nodes=10_000, n_pods=200_000, n_candidates=100, max_subset=3, n_
             i = node_pod_off[n]  # the node's first pod row
             rows_cls[i] = b.pod_class(Pod(requests=_requests(ci[order][i], mi[order][i]),
                                           node_selector={HOSTNAME_LABEL: f"node-{n:05d}"}))
+    if vol_alts > 0:
+        rest = np.setdiff1d(nonempty, cand)
+        pick = list(cand[::10]) + list(rest[::max(1, len(rest) // vol_alts)])
+        for j, n in enumerate(pick[:vol_alts]):
+            i = node_pod_off[n + 1] - 1  # the node's last pod row
+            own = zones[node_zone[n]]
+            alts = [own, zones[(node_zone[n] + 1) % len(zones)]] if j % 2 == 0 else ["no-such-zone", own]
+            rows_cls[i] = b.pod_class(Pod(requests=_requests(ci[order][i], mi[order][i]),
+                                          volume_requirements=[[NodeSelectorRequirement(ZONE_LABEL, "In", (z,))]
+                                                               for z in alts]))
     b.set_pod_arrays(rows_cls, np.zeros(len(rows_cls), np.int64), dp[order, 2], dp[order, 3])
     enc = b.build()
     subsets: List[Tuple[int, ...]] = []
